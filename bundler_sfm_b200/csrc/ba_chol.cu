@@ -7,19 +7,15 @@
 //
 //   per 32-column step : chol_step_kernel  ONE launch; every CTA redundantly factors the 32x32 diagonal
 //                        block fused with the row solves of the two panel blocks its 32x32 trailing tile
-//                        needs (8 warps, right-looking, one barrier per pivot, rsqrt + multiply on the
+//                        needs (16 warps, right-looking, one barrier per pivot, rsqrt + multiply on the
 //                        pivot chain), then applies the rank-32 update to its tile
-//   per outer panel    : chol_syrk_dmma_kernel  (systems > 1536 only) the trailing matrix beyond the 256-column
-//                        outer panel gets one K = 256 SYRK-shaped update on the fp64 tensor cores
-//                        (mma.sync m8n8k4 f64, 128x128 tiles) -- the dense contraction of this path
 //   end                : chol_backsolve_blocked_kernel (1 CTA) L^T x = y with the inverted diagonal blocks
-// This file is the dispatcher (chol_solve) and the FUSED-STEP path for systems of 641..1536 (one outer panel: latency-bound by
-// the sequential pivots).  Systems <= 640 go to the one-launch dataflow factorisation (ba_chol_dataflow.cu), systems > 1536 to
-// the 256-column panel path with the fp64 tensor-core trailing update (ba_chol_large.cu).
+// This file is the dispatcher (chol_solve) and the FUSED-STEP path for systems of 641..1536 (latency-bound by the sequential
+// pivots).  Systems <= 640 go to the one-launch dataflow factorisation (ba_chol_dataflow.cu), systems > 1536 to the 256-column
+// panel path with the fp64 tensor-core trailing update (ba_chol_large.cu).
 #include "ba_kernels.cuh"
 #include "ba_chol_large.cuh"
 #include "common.h"
-#include <cstdlib>
 
 namespace bsfm {
 namespace ba {
@@ -27,194 +23,7 @@ namespace ba {
 int chol_solve_dataflow(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *x, Scalars *sc, bool *used);
 
 constexpr int NB = 32;
-#ifdef BSFM_DEBUG_CLOCKS
-__device__ long long g_dbg[64];
-__device__ __forceinline__ long long dbg_clock() { long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t) :: "memory"); return t; }
-#define DBG_T(i) do { if (blockIdx.x == 1 && k == 0 && (threadIdx.x & 31) == 0) g_dbg[(i) + 5 * (threadIdx.x >> 5)] = dbg_clock(); } while (0)
-#else
-#define DBG_T(i) do { } while (0)
-#endif
-
-// ---- trailing update: A[r][c] -= sum_{t in [kb,ke)} A[r][t] A[c][t]  for c in [cb,ce), r >= c -----
-// square tiles BT x BT, (BT/TT)^2 = 256 threads, TT x TT outputs per thread, K chunks of 16.
-template <int BT, int TT>
-__global__ void __launch_bounds__(256) chol_syrk_kernel(double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
-{
-    constexpr int BK = 16;
-    __shared__ double As[BK][BT + 4];
-    __shared__ double Bs[BK][BT + 4];
-    const int c0 = cb + blockIdx.x * BT;
-    const int r0 = cb + blockIdx.y * BT;
-    if (r0 + BT <= c0) return;            // tile strictly above the diagonal band
-    if (c0 >= ce || r0 >= nrows) return;
-    const int tid = threadIdx.x;
-    const int tx = tid % (BT / TT), ty = tid / (BT / TT);
-    double acc[TT][TT];
-#pragma unroll
-    for (int a = 0; a < TT; a++)
-#pragma unroll
-        for (int b = 0; b < TT; b++) acc[a][b] = 0.0;
-    for (int k0 = kb; k0 < ke; k0 += BK) {
-        for (int q = tid; q < BT * BK; q += 256) {
-            const int r = q / BK, t = q % BK;
-            const int kk = k0 + t;
-            As[t][r] = (r0 + r < nrows && kk < ke) ? L[(size_t) (r0 + r) * ld + kk] : 0.0;
-            Bs[t][r] = (c0 + r < ce && kk < ke) ? L[(size_t) (c0 + r) * ld + kk] : 0.0;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int t = 0; t < BK; t++) {
-            double a[TT], b[TT];
-#pragma unroll
-            for (int q = 0; q < TT; q++) { a[q] = As[t][ty * TT + q]; b[q] = Bs[t][tx * TT + q]; }
-#pragma unroll
-            for (int qa = 0; qa < TT; qa++)
-#pragma unroll
-                for (int qb = 0; qb < TT; qb++) acc[qa][qb] = fma(a[qa], b[qb], acc[qa][qb]);
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int qa = 0; qa < TT; qa++) {
-        const int r = r0 + ty * TT + qa;
-        if (r >= nrows) continue;
-#pragma unroll
-        for (int qb = 0; qb < TT; qb++) {
-            const int c = c0 + tx * TT + qb;
-            if (c < ce && c <= r) A[(size_t) r * ld + c] -= acc[qa][qb];
-        }
-    }
-}
-
-// ---- trailing update on the fp64 tensor cores (DMMA) -----------------------------------------------
-// Same contract as chol_syrk_kernel (A[r][c] -= sum_t A[r][t] A[c][t], c in [cb,ce), r >= c), 128x128 CTA
-// tile, 8 warps as 2 (rows) x 4 (cols), warp tile 64x32 = 4x4 m16n8 accumulator tiles of mma.sync.m16n8k8.f64 (the
-// sm_90 shape: four times the work of an m8n8k4 per instruction), K chunks of 16 staged in shared memory with register
-// prefetch of the next chunk.  Both operands are rows of L (A = L, B = L^T), so one fragment pattern serves both:
-// L[row0 + lane/4 (+8)][k + lane%4 (+4)].  The output tile is prefetched into L2 when the CTA starts, so that its
-// read-modify-write at the end does not wait for HBM.
-__device__ __forceinline__ void dmma_m8n8k4(double &d0, double &d1, double a, double b)
-{
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                 : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
-}
-// D(16x8) += A(16x8) B(8x8); lane = 4 g + t holds A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4], B[t][g], B[t+4][g],
-// D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]
-__device__ __forceinline__ void dmma_m16n8k8(double (&d)[4], const double (&a)[4], const double (&b)[2])
-{
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-                 : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
-}
-
-__global__ void __launch_bounds__(256) chol_syrk_dmma_kernel(double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
-{
-    constexpr int BT = 128, BK = 16, LDS = BK + 4;
-    __shared__ double As[BT][LDS];
-    __shared__ double Bs[BT][LDS];
-    const int c0 = cb + blockIdx.x * BT;
-    const int r0 = cb + blockIdx.y * BT;
-    if (r0 + BT <= c0) return;
-    if (c0 >= ce || r0 >= nrows) return;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int wr = warp >> 2, wc = warp & 3;           // warp tile origin: rows wr*64, cols wc*32
-    const int g = lane >> 2, tg = lane & 3;
-    const bool vec2 = (ld & 1) == 0;     // 16-byte accesses need even row pitch
-    if (vec2 && tid < BT && r0 + tid < nrows) {
-        const int bytes = (min(BT, ce - c0) * 8) & ~15;
-        if (bytes > 0)
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(A + (size_t) (r0 + tid) * ld + c0), "r"(bytes) : "memory");
-    }
-    double acc[4][4][4];
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-#pragma unroll
-            for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
-
-    // global -> register prefetch: 128 rows x 16 doubles per operand = 1024 16-byte pieces, 4 per thread
-    double2 pa[4], pb[4];
-    auto fetch = [&](int k0) {
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int idx = tid + 256 * i;
-            const int row = idx >> 3, kk = k0 + (idx & 7) * 2;
-            double2 va = make_double2(0.0, 0.0), vb = make_double2(0.0, 0.0);
-            if (r0 + row < nrows) {
-                const double *src = L + (size_t) (r0 + row) * ld + kk;
-                if (kk + 1 < ke) { if (vec2) va = *reinterpret_cast<const double2 *>(src); else { va.x = src[0]; va.y = src[1]; } }
-                else if (kk < ke) va.x = src[0];
-            }
-            if (c0 + row < ce) {
-                const double *src = L + (size_t) (c0 + row) * ld + kk;
-                if (kk + 1 < ke) { if (vec2) vb = *reinterpret_cast<const double2 *>(src); else { vb.x = src[0]; vb.y = src[1]; } }
-                else if (kk < ke) vb.x = src[0];
-            }
-            pa[i] = va; pb[i] = vb;
-        }
-    };
-    auto stash = [&]() {
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int idx = tid + 256 * i;
-            const int row = idx >> 3, kc = (idx & 7) * 2;
-            *reinterpret_cast<double2 *>(&As[row][kc]) = pa[i];
-            *reinterpret_cast<double2 *>(&Bs[row][kc]) = pb[i];
-        }
-    };
-    fetch(kb);
-    for (int k0 = kb; k0 < ke; k0 += BK) {
-        __syncthreads();
-        stash();
-        __syncthreads();
-        if (k0 + BK < ke) fetch(k0 + BK);
-#pragma unroll
-        for (int ks = 0; ks < BK; ks += 8) {
-            double af[4][4], bf[4][2];
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int r = wr * 64 + i * 16 + g;
-                af[i][0] = As[r][ks + tg]; af[i][1] = As[r + 8][ks + tg];
-                af[i][2] = As[r][ks + tg + 4]; af[i][3] = As[r + 8][ks + tg + 4];
-            }
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const int c = wc * 32 + j * 8 + g;
-                bf[j][0] = Bs[c][ks + tg]; bf[j][1] = Bs[c][ks + tg + 4];
-            }
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < 4; j++) dmma_m16n8k8(acc[i][j], af[i], bf[j]);
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        const int r = r0 + wr * 64 + i * 8 + g;
-        if (r >= nrows) continue;
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int c = c0 + wc * 32 + j * 8 + 2 * tg;
-            const double v0 = acc[i >> 1][j][2 * (i & 1)], v1 = acc[i >> 1][j][2 * (i & 1) + 1];
-            double *dst = A + (size_t) r * ld + c;
-            if (vec2 && c + 1 < ce && c + 1 <= r) {
-                double2 v = *reinterpret_cast<double2 *>(dst);
-                v.x -= v0; v.y -= v1;
-                *reinterpret_cast<double2 *>(dst) = v;
-            } else {
-                if (c < ce && c <= r) dst[0] -= v0;
-                if (c + 1 < ce && c + 1 <= r) dst[1] -= v1;
-            }
-        }
-    }
-}
-
-void syrk_dmma(cudaStream_t st, double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
-{
-    constexpr int BT = 128;
-    const dim3 grid((ce - cb + BT - 1) / BT, (nrows - cb + BT - 1) / BT);
-    chol_syrk_dmma_kernel<<<grid, 256, 0, st>>>(A, L, ld, nrows, cb, ce, kb, ke);
-}
+constexpr int CHOL_LARGE_MIN = 1536;     // systems above this size are throughput-bound: 256-column panel path
 
 // ---- small systems, one launch per 32-column step ---------------------------------------------------
 // Every CTA redundantly factors the 32x32 diagonal block (one warp, rows in registers, pivots and
@@ -225,10 +34,7 @@ void syrk_dmma(cudaStream_t st, double *A, const double *L, int ld, int nrows, i
 // Row block index nbk (= one row) is the right-hand side carried along as matrix row n.
 // (loops over shared memory, not unrolled register code: a kernel this short must not spend its time
 // fetching tens of KB of straight-line instructions)
-#ifndef BSFM_CHOL_STEP_THREADS
-#define BSFM_CHOL_STEP_THREADS 512
-#endif
-constexpr int CST = BSFM_CHOL_STEP_THREADS;      // threads of chol_step_kernel (8 or 16 warps)
+constexpr int CST = 512;      // threads of chol_step_kernel
 constexpr int CSW = CST / 32;
 __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout, int ld, int n, int k, int cend, double *Linv_all, Scalars *sc)
 {
@@ -244,8 +50,7 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
     // predecessor wrote is touched before this point
     cudaGridDependencySynchronize();
     // tile of this CTA: blockIdx 0 = panel owner (no tile); else (cb, rb), k < cb <= rb <= nbk, cb < cend <= nbk
-    // (cend < nbk: only the columns of the current outer panel are updated here; the rest of the trailing matrix
-    //  is updated once per outer panel by the DMMA SYRK kernel)
+    // (cend = k + 1: the diagonal-only launch that precedes chol_tile_kernel)
     int cb = -1, rb = nbk;                        // the owner solves the RHS row segment
     bool writeback = true;
     if (blockIdx.x > 0) {
@@ -256,8 +61,8 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
             if (t < cnt) { cb = c; rb = c + t; found = true; break; }
             t -= cnt;
         }
-        // first-column tiles write their panel row block back; when the outer panel has no column left
-        // (k + 1 == cend) dedicated panel-only CTAs do it for the row blocks below
+        // first-column tiles write their panel row block back; when no column is left (k + 1 == cend)
+        // dedicated panel-only CTAs do it for the row blocks below
         if (found) writeback = (cb == k + 1); else rb = k + 1 + t;
     }
     const int crow0 = cb * NB;
@@ -269,7 +74,6 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
     const bool owner = blockIdx.x == 0;
     const bool need_c = owner || (cb >= 0 && cb != rb);
 
-    DBG_T(0);
     if (tid == 0) fail_s = 0;
     for (int e = tid; e < NB * NB; e += CST) {
         const int r = e >> 5, c = e & 31;
@@ -279,7 +83,6 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
         else if (need_c) Xc[r][c] = (r < crows && c < nb) ? A[(size_t) (crow0 + r) * ld + (k0 + c)] : 0.0;
     }
     __syncthreads();
-    DBG_T(1);
     // potf2 of L_kk fused with the row solves X <- X L_kk^-T, right-looking, all 8 warps:
     //   thread (lane r, warp g) owns rows r and columns c = g, g+8, g+16, g+24.
     //   Every warp recomputes the pivot reciprocal and the multipliers l_r = a_rj / sqrt(d) of column j
@@ -311,7 +114,6 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
     }
     if (tid < NB && tid >= nb) dinv[tid] = 1.0;
     __syncthreads();
-    DBG_T(2);
     // rescale: L[r][c] = a_rc dinv[c] (c < r), L[c][c] = d_c dinv[c], X[r][c] *= dinv[c]
     for (int e = tid; e < NB * NB; e += CST) {
         const int r = e >> 5, c = e & 31;
@@ -326,7 +128,6 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
         if (lane == 0 && fail_s) sc->chol_fail = 1;
     }
     __syncthreads();
-    DBG_T(3);
     if (owner) {   // Z = L_kk^-1 = Xc^T (lower triangular)
         for (int e = tid; e < NB * NB; e += CST) { const int r = e >> 5, c = e & 31; Linv_all[(size_t) k * NB * NB + e] = (c <= r) ? Xc[c][r] : 0.0; }
     }
@@ -353,7 +154,6 @@ __global__ void __launch_bounds__(CST) chol_step_kernel(double *A, double *Lout,
             A[(size_t) (rbase + r) * ld + (crow0 + c)] -= acc;
         }
     }
-    DBG_T(4);
 }
 
 // ---- large grids: tile kernel that takes L_kk^-1 from a preceding diagonal-only chol_step launch -------
@@ -510,61 +310,34 @@ __global__ void __launch_bounds__(512) chol_backsolve_blocked_kernel(const doubl
 // linv_ws: ceil(n/32) * 1024 doubles (+ n doubles of back-substitution workspace behind it).
 int chol_solve(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *x, Scalars *sc)
 {
-    // systems beyond the latency-bound regime: 256-column panels, fp64 tensor-core trailing update (ba_chol_large.cu);
-    // BSFM_BA_CHOL_LARGE_MIN moves the switch-over (tests run the large path on small systems with it)
-    static const int large_min = []() { const char *e = getenv("BSFM_BA_CHOL_LARGE_MIN"); return e ? atoi(e) : 1536; }();
-    static const bool old_large = getenv("BSFM_BA_CHOL_OLD") != nullptr;      // the 32-column-step path with the DMMA update for large systems too, kept for A/B timing
-    if (n <= large_min && n > LNB) {      // small systems: one co-resident dataflow launch per factorisation (ba_chol_dataflow.cu)
+    const int nbk = (n + NB - 1) / NB;
+    if (n > CHOL_LARGE_MIN) return chol_solve_large(st, A, Lmat, n, linv_ws, linv_ws + (size_t) nbk * NB * NB, x, sc);
+    if (n > LNB) {      // small systems: one co-resident dataflow launch per factorisation (ba_chol_dataflow.cu)
         bool used = false;
         int rc = chol_solve_dataflow(st, A, Lmat, n, linv_ws, x, sc, &used);
         if (rc != BSFM_OK || used) return rc;
     }
-    if (n > large_min && !old_large) return chol_solve_large(st, A, Lmat, n, linv_ws, linv_ws + (size_t) ((n + NB - 1) / NB) * NB * NB, x, sc);
-    const int ld = n, nrows = n + 1;
-    const int nbk = (n + NB - 1) / NB;
+    const int ld = n;
     double *ywork = linv_ws + (size_t) nbk * NB * NB;
-    // outer panels of NBO columns: inside a panel one fused chol_step launch per 32 columns touches only the
-    // panel's own columns; the rest of the trailing matrix gets ONE K = NBO update on the fp64 tensor cores.
-    // Small systems (latency-bound) use a single outer panel = the whole matrix.
-    const int NBO = (n > 1536) ? 256 : nbk * NB;
-    static const bool use_pdl = getenv("BSFM_BA_NO_PDL") == nullptr;
-    for (int K0 = 0; K0 < n; K0 += NBO) {
-        const int K1 = min(n, K0 + NBO);
-        const int cend = (K1 + NB - 1) / NB;
-        for (int k = K0 / NB; k < cend; k++) {
-            int tiles = 0;
-            for (int c = k + 1; c < cend; c++) tiles += nbk - c + 1;
-            const int extra = (k + 1 >= cend) ? (nbk - 1 - k) : 0;
-            if (tiles + extra > 800) {
-                // many more tiles than resident CTAs: factor the diagonal block once, then the GEMM-style tile kernel
-                chol_step_kernel<<<1, CST, 0, st>>>(A, Lmat, ld, n, k, k + 1, linv_ws, sc);
-                BSFM_KERNEL_CHECK();
-                chol_tile_kernel<<<tiles + extra, 256, 0, st>>>(A, Lmat, ld, n, k, cend, linv_ws);
-                BSFM_KERNEL_CHECK();
-            } else {
-                if (use_pdl) { BSFM_CUDA_TRY(launch_pdl(chol_step_kernel, dim3(1 + tiles + extra), dim3(CST), st, A, Lmat, ld, n, k, cend, linv_ws, sc)); count_launch(); }
-                else { chol_step_kernel<<<1 + tiles + extra, CST, 0, st>>>(A, Lmat, ld, n, k, cend, linv_ws, sc); BSFM_KERNEL_CHECK(); }
-            }
-        }
-        if (K1 < n) {
-            const int BT = 128;
-            dim3 grid((n - K1 + BT - 1) / BT, (nrows - K1 + BT - 1) / BT);
-            if (getenv("BSFM_BA_NO_DMMA")) chol_syrk_kernel<128, 8><<<grid, 256, 0, st>>>(A, Lmat, ld, nrows, K1, n, K0, K1);
-            else syrk_dmma(st, A, Lmat, ld, nrows, K1, n, K0, K1);
+    // one fused chol_step launch per 32 columns over the whole trailing matrix
+    for (int k = 0; k < nbk; k++) {
+        int tiles = 0;
+        for (int c = k + 1; c < nbk; c++) tiles += nbk - c + 1;
+        if (tiles > 800) {
+            // many more tiles than resident CTAs: factor the diagonal block once, then the GEMM-style tile kernel
+            chol_step_kernel<<<1, CST, 0, st>>>(A, Lmat, ld, n, k, k + 1, linv_ws, sc);
             BSFM_KERNEL_CHECK();
+            chol_tile_kernel<<<tiles, 256, 0, st>>>(A, Lmat, ld, n, k, nbk, linv_ws);
+            BSFM_KERNEL_CHECK();
+        } else {
+            BSFM_CUDA_TRY(launch_pdl(chol_step_kernel, dim3(1 + tiles), dim3(CST), st, A, Lmat, ld, n, k, nbk, linv_ws, sc));
+            count_launch();
         }
     }
-    if (use_pdl) { BSFM_CUDA_TRY(launch_pdl(chol_backsolve_blocked_kernel, dim3(1), dim3(512), st, (const double *) Lmat, ld, n, (const double *) linv_ws, x, ywork)); count_launch(); }
-    else { chol_backsolve_blocked_kernel<<<1, 512, 0, st>>>(Lmat, ld, n, linv_ws, x, ywork); BSFM_KERNEL_CHECK(); }
+    BSFM_CUDA_TRY(launch_pdl(chol_backsolve_blocked_kernel, dim3(1), dim3(512), st, (const double *) Lmat, ld, n, (const double *) linv_ws, x, ywork));
+    count_launch();
     return BSFM_OK;
 }
 
 }  // namespace ba
 }  // namespace bsfm
-
-#ifdef BSFM_DEBUG_CLOCKS
-extern "C" int bsfm_debug_read(long long *out64)
-{
-    return cudaMemcpyFromSymbol(out64, bsfm::ba::g_dbg, sizeof(long long) * 64) == cudaSuccess ? 0 : -2;
-}
-#endif

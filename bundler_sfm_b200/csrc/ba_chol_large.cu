@@ -9,7 +9,7 @@
 //                                 in-block update) + the inverses of its eight 32 x 32 diagonal sub-blocks
 //   chol_trsm_kernel      64 rows x 256 columns per CTA : L_panel = A_panel L_kk^-T as a blocked forward substitution
 //                                 (small GEMMs against the sub-block inverses)
-//   chol_syrk_dmma_kernel A -= L_panel L_panel^T, K = 256, on the fp64 tensor cores (ba_chol.cu)
+//   chol_syrk_dmma_kernel A -= L_panel L_panel^T, K = 256, on the fp64 tensor cores
 //   (after the last panel) chol_backsolve_big_kernel per panel, last to first: L^T x = y
 // The small-system path (ba_chol.cu: one fused launch per 32 columns) stays as it is: it is latency-bound, this one is
 // throughput-bound.
@@ -49,10 +49,8 @@ constexpr int DG_XROWS = LNBO - LNB;          // 224 panel rows at most inside t
 constexpr int DG_SMEM_DOUBLES = (3 * LNB + DG_XROWS) * DG_LD + LNB;
 static_assert(DG_LD == TP, "tile primitives of ba_chol_potf2.cuh use a pitch of 36 doubles");
 constexpr int DG_THREADS = 256;    // 255 registers per thread: the register-resident 32-wide rows need them
-__global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, double *Lout, int ld, int n, int k0, double *linv_all, Scalars *sc, long long *dbg)
+__global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, double *Lout, int ld, int n, int k0, double *linv_all, Scalars *sc)
 {
-#define DG_T(i) do { if (dbg && tid == 0) { const long long now = clock64(); dbg[i] += now - tlast; tlast = now; } } while (0)
-    long long tlast = dbg ? clock64() : 0;
     extern __shared__ __align__(16) double dsm[];
     double (*Ls)[DG_LD] = reinterpret_cast<double (*)[DG_LD]>(dsm);
     double (*Zs)[DG_LD] = reinterpret_cast<double (*)[DG_LD]>(dsm + LNB * DG_LD);
@@ -87,23 +85,17 @@ __global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, dou
             }
         }
         __syncthreads();
-        DG_T(0);
         if (warp == 0) {
             // potf2 of the 32 x 32 block (ba_chol_potf2.cuh): lane = row, 8-column register panels, DMMA rank-8 updates
             const bool bad = warp_potf2_32_tc(Ls, dinv, lane, true);
             if (bad && lane == 0) sc->chol_fail = 1;
-            DG_T(5);                                            // dev accounting: potf2 alone; slot 1 is then the wait for the inverse
         } else if (warp == 1) {
-            const long long t1 = dbg ? clock64() : 0;
             warp_tile_inverse(Ls, dinv, Zs, Ws, lane);          // Z = L_ss^-1 assembled one panel behind warp 0
-            if (dbg && lane == 0) dbg[6] += clock64() - t1;
         }
         __syncthreads();
-        DG_T(1);
         // panel rows below the sub-block: X <- X L_ss^-T = X Z^T, 8-row strips on the fp64 tensor cores
         for (int strip = warp; strip * 8 < below; strip += DG_THREADS / 32) warp_rows_times_ZT(Xs, strip * 8, Zs, lane);
         __syncthreads();
-        DG_T(2);
         for (int e = tid; e < LNB * LNB; e += DG_THREADS) {
             const int r = e >> 5, c = e & 31;
             if (r < w && c <= r) Lout[(size_t) (c0 + r) * ld + (c0 + c)] = Ls[r][c];
@@ -113,7 +105,6 @@ __global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, dou
             const int r = e >> 5, c = e & 31;
             if (c < w) Lout[(size_t) (c0 + LNB + r) * ld + (c0 + c)] = Xs[r][c];
         }
-        DG_T(3);
         // rank-32 update of the remaining block: tile (bi, bj), bj <= bi, on the fp64 tensor cores
         for (int blk = warp; blk < nblk * (nblk + 1) / 2; blk += DG_THREADS / 32) {
             int bi = 0, rem = blk;
@@ -158,9 +149,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, dou
             }
         }
         __syncthreads();
-        DG_T(4);
     }
-#undef DG_T
 }
 
 // ---- panel solve: rows below the diagonal block (and the right-hand side row n) ----------------------------------
@@ -300,6 +289,131 @@ __global__ void __launch_bounds__(256) chol_trsm_kernel(const TrsmArgs T)
     }
 }
 
+// ---- trailing update on the fp64 tensor cores (DMMA) -----------------------------------------------
+// A[r][c] -= sum_{t in [kb,ke)} L[r][t] L[c][t]  for c in [cb,ce), r in [c, nrows).  128x128 CTA
+// tile, 8 warps as 2 (rows) x 4 (cols), warp tile 64x32 = 4x4 m16n8 accumulator tiles of mma.sync.m16n8k8.f64 (the
+// sm_90 shape: four times the work of an m8n8k4 per instruction), K chunks of 16 staged in shared memory with register
+// prefetch of the next chunk.  Both operands are rows of L (A = L, B = L^T), so one fragment pattern serves both:
+// L[row0 + lane/4 (+8)][k + lane%4 (+4)].  The output tile is prefetched into L2 when the CTA starts, so that its
+// read-modify-write at the end does not wait for HBM.
+// D(16x8) += A(16x8) B(8x8); lane = 4 g + t holds A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4], B[t][g], B[t+4][g],
+// D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]
+__device__ __forceinline__ void dmma_m16n8k8(double (&d)[4], const double (&a)[4], const double (&b)[2])
+{
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
+
+__global__ void __launch_bounds__(256) chol_syrk_dmma_kernel(double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
+{
+    constexpr int BT = 128, BK = 16, LDS = BK + 4;
+    __shared__ double As[BT][LDS];
+    __shared__ double Bs[BT][LDS];
+    const int c0 = cb + blockIdx.x * BT;
+    const int r0 = cb + blockIdx.y * BT;
+    if (r0 + BT <= c0) return;
+    if (c0 >= ce || r0 >= nrows) return;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wr = warp >> 2, wc = warp & 3;           // warp tile origin: rows wr*64, cols wc*32
+    const int g = lane >> 2, tg = lane & 3;
+    const bool vec2 = (ld & 1) == 0;     // 16-byte accesses need even row pitch
+    if (vec2 && tid < BT && r0 + tid < nrows) {
+        const int bytes = (min(BT, ce - c0) * 8) & ~15;
+        if (bytes > 0)
+            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(A + (size_t) (r0 + tid) * ld + c0), "r"(bytes) : "memory");
+    }
+    double acc[4][4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+#pragma unroll
+            for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
+
+    // global -> register prefetch: 128 rows x 16 doubles per operand = 1024 16-byte pieces, 4 per thread
+    double2 pa[4], pb[4];
+    auto fetch = [&](int k0) {
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int idx = tid + 256 * i;
+            const int row = idx >> 3, kk = k0 + (idx & 7) * 2;
+            double2 va = make_double2(0.0, 0.0), vb = make_double2(0.0, 0.0);
+            if (r0 + row < nrows) {
+                const double *src = L + (size_t) (r0 + row) * ld + kk;
+                if (kk + 1 < ke) { if (vec2) va = *reinterpret_cast<const double2 *>(src); else { va.x = src[0]; va.y = src[1]; } }
+                else if (kk < ke) va.x = src[0];
+            }
+            if (c0 + row < ce) {
+                const double *src = L + (size_t) (c0 + row) * ld + kk;
+                if (kk + 1 < ke) { if (vec2) vb = *reinterpret_cast<const double2 *>(src); else { vb.x = src[0]; vb.y = src[1]; } }
+                else if (kk < ke) vb.x = src[0];
+            }
+            pa[i] = va; pb[i] = vb;
+        }
+    };
+    auto stash = [&]() {
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int idx = tid + 256 * i;
+            const int row = idx >> 3, kc = (idx & 7) * 2;
+            *reinterpret_cast<double2 *>(&As[row][kc]) = pa[i];
+            *reinterpret_cast<double2 *>(&Bs[row][kc]) = pb[i];
+        }
+    };
+    fetch(kb);
+    for (int k0 = kb; k0 < ke; k0 += BK) {
+        __syncthreads();
+        stash();
+        __syncthreads();
+        if (k0 + BK < ke) fetch(k0 + BK);
+#pragma unroll
+        for (int ks = 0; ks < BK; ks += 8) {
+            double af[4][4], bf[4][2];
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const int r = wr * 64 + i * 16 + g;
+                af[i][0] = As[r][ks + tg]; af[i][1] = As[r + 8][ks + tg];
+                af[i][2] = As[r][ks + tg + 4]; af[i][3] = As[r + 8][ks + tg + 4];
+            }
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const int c = wc * 32 + j * 8 + g;
+                bf[j][0] = Bs[c][ks + tg]; bf[j][1] = Bs[c][ks + tg + 4];
+            }
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) dmma_m16n8k8(acc[i][j], af[i], bf[j]);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const int r = r0 + wr * 64 + i * 8 + g;
+        if (r >= nrows) continue;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int c = c0 + wc * 32 + j * 8 + 2 * tg;
+            const double v0 = acc[i >> 1][j][2 * (i & 1)], v1 = acc[i >> 1][j][2 * (i & 1) + 1];
+            double *dst = A + (size_t) r * ld + c;
+            if (vec2 && c + 1 < ce && c + 1 <= r) {
+                double2 v = *reinterpret_cast<double2 *>(dst);
+                v.x -= v0; v.y -= v1;
+                *reinterpret_cast<double2 *>(dst) = v;
+            } else {
+                if (c < ce && c <= r) dst[0] -= v0;
+                if (c + 1 < ce && c + 1 <= r) dst[1] -= v1;
+            }
+        }
+    }
+}
+
+static void syrk_dmma(cudaStream_t st, double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
+{
+    constexpr int BT = 128;
+    const dim3 grid((ce - cb + BT - 1) / BT, (nrows - cb + BT - 1) / BT);
+    chol_syrk_dmma_kernel<<<grid, 256, 0, st>>>(A, L, ld, nrows, cb, ce, kb, ke);
+}
+
 // ---- back substitution L^T x = y, one launch per outer panel (last to first) --------------------------------------
 // y lives in row n of the factor matrix and is updated in place.  Every CTA first forms the panel's own 256 unknowns
 // x_p = L_pp^-T y_p with the inverse computed after the factorisation (Xinv = L_pp^-T, row-major 256 x 256, upper
@@ -383,7 +497,6 @@ struct CholProfile {
 thread_local CholProfile g_prof;
 }  // namespace
 
-static long long *g_diag_dbg = nullptr;     // dev-only (BSFM_DIAG_PROF=1): cycles of the first panel's diagonal-block phases
 static int set_smem_attr_once(int dev)
 {
     static std::atomic<int> done[64];
@@ -403,8 +516,6 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
     int dev = 0;
     BSFM_CUDA_TRY(cudaGetDevice(&dev));
     { int rc = set_smem_attr_once(dev); if (rc != BSFM_OK) return rc; }
-    static const bool diag_prof = getenv("BSFM_DIAG_PROF") != nullptr;
-    if (diag_prof && !g_diag_dbg) { cudaMalloc(&g_diag_dbg, 8 * sizeof(long long)); cudaMemset(g_diag_dbg, 0, 8 * sizeof(long long)); }
     // Look-ahead: the diagonal block of panel p+1 is a serial chain on ONE SM.  The trailing update of panel p is therefore
     // split into the tile columns panel p+1 lives in (launched first) and the rest, and diag(p+1) runs on a side stream next
     // to the rest, taking the first SM the rest's CTAs leave free:
@@ -441,7 +552,7 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
         }
         if (!diag_done) {
             g_prof.begin(0, st);
-            chol_diag_kernel<<<1, DG_THREADS, DG_SMEM_DOUBLES * sizeof(double), st>>>(A, Lmat, ld, n, k0, linv_ws, sc, k0 == 0 ? g_diag_dbg : nullptr);
+            chol_diag_kernel<<<1, DG_THREADS, DG_SMEM_DOUBLES * sizeof(double), st>>>(A, Lmat, ld, n, k0, linv_ws, sc);
             BSFM_KERNEL_CHECK();
             g_prof.end(st);
         } else {
@@ -467,7 +578,7 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
                 BSFM_KERNEL_CHECK();
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_col, st));
                 BSFM_CUDA_TRY(cudaStreamWaitEvent(side.st, side.e_col, 0));
-                chol_diag_kernel<<<1, DG_THREADS, DG_SMEM_DOUBLES * sizeof(double), side.st>>>(A, Lmat, ld, n, k1, linv_ws, sc, nullptr);
+                chol_diag_kernel<<<1, DG_THREADS, DG_SMEM_DOUBLES * sizeof(double), side.st>>>(A, Lmat, ld, n, k1, linv_ws, sc);
                 BSFM_KERNEL_CHECK();
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_diag, side.st));
                 diag_done = true;
@@ -520,12 +631,4 @@ extern "C" int bsfm_ba_chol_profile_read(float ms[4], int launches[4], double *f
     for (int q = 0; q < 4; q++) { if (ms) ms[q] = g_prof.ms[q]; if (launches) launches[q] = g_prof.launches[q]; }
     if (fp64_flops) *fp64_flops = g_prof.fp64_flops;
     return BSFM_OK;
-}
-
-extern "C" int bsfm_debug_diag_prof(long long *out8)
-{
-    if (!bsfm::ba::g_diag_dbg) return -1;
-    if (cudaMemcpy(out8, bsfm::ba::g_diag_dbg, 8 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return -2;
-    cudaMemset(bsfm::ba::g_diag_dbg, 0, 8 * sizeof(long long));
-    return 0;
 }

@@ -12,11 +12,10 @@ struct Scalars;
 
 constexpr int LNB = 32;          // sub-block
 constexpr int LNBO = 256;        // outer panel
-// A[r][c] -= sum_{t in [kb,ke)} L[r][t] L[c][t]  for c in [cb,ce), r in [c, nrows), on the fp64 tensor cores (ba_chol.cu)
-void syrk_dmma(cudaStream_t st, double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke);
 int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *xinv_ws, double *x, Scalars *sc);
 // doubles of linear-solver workspace behind the 32 x 32 inverses: back-substitution scratch (small path) or the 256 x 256 panel inverses (large path)
 constexpr int DF_MAX_N = 24 * LNB;       // largest system the dataflow path (ba_chol_dataflow.cu) takes: it needs (n + 1) x n doubles more
+constexpr int DF_MAX_NBK = 20;           // and at most this many 32-column blocks (n <= 640)
 inline size_t chol_extra_ws_doubles(int n)
 {
     // small systems: (n + 1) x n behind the scratch; large ones finish their last panels with the dataflow kernel: room for its largest case

@@ -184,11 +184,10 @@ struct HostMarks {
 };
 
 #define TRY(expr) do { int rc__ = (expr); if (rc__ != BSFM_OK) return rc__; } while (0)
-// PDL launch of a BA kernel on stream `st` (plain launch when BSFM_BA_NO_PDL is set)
+// PDL launch of a BA kernel on stream `st`
 #define BA_LAUNCH(kernel, grid, block, ...)                                                              \
     do {                                                                                                \
-        if (use_pdl) BSFM_CUDA_TRY(launch_pdl(kernel, dim3(grid), dim3(block), st, __VA_ARGS__));       \
-        else kernel<<<(grid), (block), 0, st>>>(__VA_ARGS__);                                          \
+        BSFM_CUDA_TRY(launch_pdl(kernel, dim3(grid), dim3(block), st, __VA_ARGS__));                    \
         BSFM_KERNEL_CHECK();                                                                            \
     } while (0)
 
@@ -224,7 +223,6 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
         if (jm && !strcmp(jm, "fd")) jac_mode = BSFM_BA_JAC_FD;
     }
     { int dev = 0; BSFM_CUDA_TRY(cudaGetDevice(&dev)); g_pool.bind_device(dev); }
-    static const bool use_pdl = getenv("BSFM_BA_NO_PDL") == nullptr;
     const long long launches0 = g_kernel_launches.load();
     // stream, events and the pinned scalar blocks are created once per thread and device and reused: driver
     // calls that allocate (cudaMallocHost, cudaStreamCreate, ...) serialise on a global lock and cost more than

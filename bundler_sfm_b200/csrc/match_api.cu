@@ -422,7 +422,7 @@ static int64_t match_run_impl(bsfm_keydb *db, int img_begin, int img_end, int wi
             BSFM_KERNEL_CHECK();
             BSFM_CUDA_TRY(cudaEventRecord(db->ev[2], db->stream));
         } else {
-            const int grid = (int) std::min<int64_t>(env_int("BSFM_MATCH_GRID", db->num_sms), u1 - u0);   // env: dev experiments only
+            const int grid = (int) std::min<int64_t>(db->num_sms, u1 - u0);
             if (P.epi_mode == 1 && pair_mode && (u1 - u0) % 2 == 0) {
                 cudaLaunchConfig_t cfg = {};
                 cfg.gridDim = dim3((unsigned) (2 * std::min<int64_t>(std::max(1, db->num_sms / 2), (u1 - u0) / 2)));
@@ -609,7 +609,7 @@ int64_t bsfm_match_all_pairs(const uint8_t *keys, const int64_t *key_off, int nu
  * (src/KeyMatchFull.cpp:105-151: keys live for the whole run, SURVEY.md 8b).  Prepared device images (norm-sorted,
  * swizzled) are therefore cached per (host pointer, key count, 64-bit content hash): a repeated image costs one hash of
  * its 640 KB instead of an upload, ~10 cudaMallocs and a segmented sort, and the pair runs on a persistent two-image
- * database filled by device-to-device copies.  BSFM_MATCH_PAIR_CACHE=0 restores the build-per-call path. */
+ * database filled by device-to-device copies. */
 namespace {
 struct CachedImage { const uint8_t *host; int n; uint64_t hash; bsfm_keydb *db; uint64_t last_use; size_t bytes; };
 struct PairCache {
@@ -754,25 +754,7 @@ int bsfm_match_pair_test(const uint8_t *k1, int n1, const uint8_t *k2, int n2, d
     int rc = require_device();
     if (rc != BSFM_OK) return rc;
     if (n1 == 0 || n2 == 0) return 0;
-    if (env_int("BSFM_MATCH_PAIR_CACHE", 1) != 0 || ratio_test != BSFM_RATIO_TEST_KEYS2A) return match_pair_cached(k1, n1, k2, n2, ratio, ratio_test, out_pairs, cap);
-    std::vector<uint8_t> keys((size_t) (n1 + n2) * DESC_BYTES);
-    memcpy(keys.data(), k1, (size_t) n1 * DESC_BYTES);
-    memcpy(keys.data() + (size_t) n1 * DESC_BYTES, k2, (size_t) n2 * DESC_BYTES);
-    int64_t off[3] = {0, n1, (int64_t) n1 + n2};
-    bsfm_keydb *db = bsfm_keydb_create(keys.data(), off, 2);
-    if (!db) return BSFM_ERR_CUDA;
-    int64_t total = bsfm_match_run(db, 1, 2, -1, ratio);
-    if (total > 0) {
-        std::vector<int32_t> m((size_t) total * 2);
-        int32_t pc = 0;
-        rc = bsfm_match_fetch(db, &pc, 1, m.data(), total);
-        if (rc != BSFM_OK) { bsfm_keydb_destroy(db); return rc; }
-        int64_t ncopy = std::min<int64_t>(total, cap);
-        if (ncopy > 0 && out_pairs) memcpy(out_pairs, m.data(), (size_t) ncopy * 2 * sizeof(int32_t));
-    }
-    bsfm_keydb_destroy(db);
-    if (total > INT_MAX) total = INT_MAX;
-    return (int) total;
+    return match_pair_cached(k1, n1, k2, n2, ratio, ratio_test, out_pairs, cap);
 }
 
 /* ---- multi-GPU behind the C ABI (SURVEY.md 8e; KeyMatchFull.cpp:105-151 sharded by database image) --------------------- */

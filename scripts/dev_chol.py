@@ -1,5 +1,5 @@
 """dev: time and check bsfm_sba_Axb_Chol on random SPD systems (run on the GPU box).
-usage: python scripts/dev_chol.py [sizes...]      env: BSFM_BA_CHOL_OLD=1"""
+usage: python scripts/dev_chol.py [sizes...]"""
 import ctypes
 import os
 import sys
@@ -28,7 +28,6 @@ def main():
     fn = lib.bsfm_sba_Axb_Chol_timed
     fn.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float)]
     fn.restype = ctypes.c_int
-    tag = f"OLD={os.environ.get('BSFM_BA_CHOL_OLD', '0')}"
     for n in sizes:
         A = spd(n, seed=n)
         rng = np.random.default_rng(1)
@@ -39,30 +38,22 @@ def main():
         rc = fn(A.ctypes.data, b.ctypes.data, x.ctypes.data, n, 1, ctypes.byref(ms))          # warm-up (allocations, attributes)
         reps = 5 if n >= 4000 else 20
         rc = fn(A.ctypes.data, b.ctypes.data, x.ctypes.data, n, reps, ctypes.byref(ms))
-        if n > 1536 and os.environ.get("BSFM_BA_CHOL_OLD") is None:
-            if os.environ.get("BSFM_DIAG_PROF"):
-                lib.bsfm_debug_diag_prof((ctypes.c_int64 * 8)())     # reset
+        if n > 1536:
             lib.bsfm_ba_chol_profile(1)
             m2 = ctypes.c_float(0)
             fn(A.ctypes.data, b.ctypes.data, x.ctypes.data, n, 3, ctypes.byref(m2))
             pms = (ctypes.c_float * 4)(); pl = (ctypes.c_int * 4)(); fl = ctypes.c_double()
             lib.bsfm_ba_chol_profile_read(pms, pl, ctypes.byref(fl))
             lib.bsfm_ba_chol_profile(0)
-            if os.environ.get("BSFM_DIAG_PROF"):
-                dp = (ctypes.c_int64 * 8)()
-                if lib.bsfm_debug_diag_prof(dp) == 0:
-                    v = [x / 3 / 1.9e3 for x in dp]     # 3 solves since the reset, us at 1.9 GHz
-                    print(f"    diag panel 0 (us, approx): load {v[0]:.1f}  potf2 {v[1]:.1f}  rowsolve+inv {v[2]:.1f}  store {v[3]:.1f}  trailing {v[4]:.1f} | potf2 alone {v[5]:.1f}  inverse warp (incl. waits) {v[6]:.1f}", flush=True)
             print(f"    per solve: diag {pms[0]/3:.3f} ms ({pl[0]//3} launches)  trsm {pms[1]/3:.3f} ms  trailing {pms[2]/3:.3f} ms "
                   f"({fl.value/3/(pms[2]/3*1e-3)/1e12:.1f} TF/s fp64)  backsolve {pms[3]/3:.3f} ms", flush=True)
-        if os.environ.get("BSFM_DF_PROF") and hasattr(lib, "bsfm_debug_df_prof"):
-            dp = (ctypes.c_uint64 * 8)()
-            if lib.bsfm_debug_df_prof(dp) == 0 and dp[7]:
-                v = list(dp); st = max(v[6], 1)
-                print(f"    dataflow CTA0: kernel {v[0]/v[7]/1e3:.1f} us/launch; cycles/step: potf2 {v[1]/st:.0f}  barrier {v[2]/st:.0f}  strips+wait-for-inputs {v[3]/st:.0f}  "
-                      f"update {v[4]/st:.0f}  end-barrier {v[5]/st:.0f}  ({v[6]} steps, {v[7]} launches)", flush=True)
+        dp = (ctypes.c_uint64 * 8)()
+        if lib.bsfm_debug_df_prof(dp) == 0 and dp[7]:
+            v = list(dp); st = max(v[6], 1)
+            print(f"    dataflow CTA0: kernel {v[0]/v[7]/1e3:.1f} us/launch; cycles/step: potf2 {v[1]/st:.0f}  barrier {v[2]/st:.0f}  strips+wait-for-inputs {v[3]/st:.0f}  "
+                  f"update {v[4]/st:.0f}  end-barrier {v[5]/st:.0f}  ({v[6]} steps, {v[7]} launches)", flush=True)
         if rc != 1:
-            print(f"[{tag}] n={n}: rc={rc} err={lib.bsfm_last_error()}")
+            print(f"n={n}: rc={rc} err={lib.bsfm_last_error()}")
             continue
         t0 = time.perf_counter()
         xr = np.linalg.solve(A, b)
@@ -73,7 +64,7 @@ def main():
         errt = np.linalg.norm(x - xt) / np.linalg.norm(xt)
         errt_ref = np.linalg.norm(xr - xt) / np.linalg.norm(xt)
         tf = (n ** 3 / 3.0 + 2.0 * n * n) / (ms.value * 1e-3) / 1e12
-        print(f"[{tag}] n={n}: {ms.value:8.3f} ms  {tf:6.2f} TF/s(fp64-equiv)  resid={res:.2e} (lapack {res_ref:.2e})  |x-x_lapack|/|x|={err:.2e}  "
+        print(f"n={n}: {ms.value:8.3f} ms  {tf:6.2f} TF/s(fp64-equiv)  resid={res:.2e} (lapack {res_ref:.2e})  |x-x_lapack|/|x|={err:.2e}  "
               f"err_vs_truth={errt:.2e} (lapack {errt_ref:.2e})  cpu={tcpu*1e3:.0f} ms", flush=True)
 
 
