@@ -9,7 +9,8 @@
 //                                 in-block update) + the inverses of its eight 32 x 32 diagonal sub-blocks
 //   chol_trsm_kernel      64 rows x 256 columns per CTA : L_panel = A_panel L_kk^-T as a blocked forward substitution
 //                                 (small GEMMs against the sub-block inverses)
-//   chol_syrk_dmma_kernel A -= L_panel L_panel^T, K = 256, on the fp64 tensor cores
+//   chol_syrk_dmma_kernel A -= L_panel L_panel^T, K = 256, on the fp64 tensor cores: persistent, warp-specialised, fed
+//                                 by TMA from a pre-tiled image of the panel that chol_trsm_kernel writes
 //   (after the last panel) chol_backsolve_big_kernel per panel, last to first: L^T x = y
 // The small-system path (ba_chol.cu: one fused launch per 32 columns) stays as it is: it is latency-bound, this one is
 // throughput-bound.
@@ -17,6 +18,7 @@
 #include "ba_chol_large.cuh"
 #include "ba_chol_potf2.cuh"
 #include "common.h"
+#include "tc_ptx.cuh"
 #include <algorithm>
 #include <atomic>
 #include <cstdlib>
@@ -152,6 +154,33 @@ __global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, dou
     }
 }
 
+// ---- pre-tiled panel image: the operands of the trailing update --------------------------------------------------
+// Written by chol_trsm_kernel next to the panel in Lmat: image row q is matrix row k1 + q (the rows
+// below the diagonal block, right-hand side row n included), stored as blocks of 128 rows x 32 k, each the exact shared-memory
+// image of one operand stage (32 KB): block (q / 128, c / 32) starts at ((q / 128) * 8 + c / 32) * 4096 doubles, whatever the
+// matrix pitch.  Inside a block, row r is 16 units of 16 bytes; k = 8 s + 4 h + t (k8 step s, half h, t = k & 3) is element h
+// of unit  u = 4 t + (s ^ (t >> 1) ^ 2 (r & 1)).  So one 16-byte load gives a lane both values (t, t + 4) of an m16n8k8
+// fragment row, and the XOR spreads the eight lanes of every quarter warp (rows g, g + 1 for even g; t = 0..3) over the
+// eight 16-byte bank groups: the fragment loads are free of bank conflicts without padding
+// (tests/test_chol_trailing_swizzle.py enumerates them).
+constexpr int SY_BT = 128, SY_BK = 32, SY_KCH = LNBO / SY_BK;      // tile, K chunk, chunks per panel
+constexpr int SY_BLOCK = SY_BT * SY_BK;                             // doubles per operand stage (32 KB)
+constexpr int SY_STAGES = 3;
+constexpr int SY_CONSUMERS = 8, SY_THREADS = 32 * (SY_CONSUMERS + 4);      // two consumer warpgroups + the producer's
+// Registers: 168 per thread at launch (384 threads, one CTA per SM); the producer warpgroup gives 128 of them back and the
+// consumers take them: 4 warps x 40 + 8 warps x 232 = 12 warps x 168
+constexpr int SY_PRODUCER_REGS = 40, SY_CONSUMER_REGS = 232;
+constexpr size_t SY_SMEM = (size_t) SY_STAGES * 2 * SY_BLOCK * sizeof(double) + 2 * SY_STAGES * 8;
+__device__ __forceinline__ size_t syrk_img_index(int q, int c)
+{
+    const int r = q & (SY_BT - 1), k = c & (SY_BK - 1), t = k & 3;
+    const int u = 4 * t + ((k >> 3) ^ (t >> 1) ^ ((r & 1) << 1));
+    return ((size_t) (q / SY_BT) * SY_KCH + c / SY_BK) * SY_BLOCK + r * SY_BK + 2 * u + ((k >> 2) & 1);
+}
+// doubles of the image of the first panel (the largest); it lives in xinv_ws, which holds ceil(n/256) * 65536 doubles and is
+// not used before the factorisation ends: ceil((n - 255) / 128) <= 2 ceil(n / 256), so it always fits
+static size_t syrk_img_doubles(int n) { return (size_t) ((n + 1 - LNBO + SY_BT - 1) / SY_BT) * SY_KCH * SY_BLOCK; }
+
 // ---- panel solve: rows below the diagonal block (and the right-hand side row n) ----------------------------------
 // X_s = (B_s - sum_{t<s} X_t L_st^T) Z_ss^T for the eight 32-column sub-blocks s, 64 rows per CTA, X kept in shared
 // memory, every product on the fp64 tensor cores (DMMA): warp (wr = warp & 3, wc = warp >> 2) owns the 16 x 16 piece
@@ -166,6 +195,7 @@ constexpr int TR_SMEM_DOUBLES = TR_ROWS * TR_LDX + TR_NLB * LNB * TR_LDB;
 struct TrsmArgs {
     const double *A;        // ident == 0: source rows (matrix, pitch ld)
     double *dst;            // destination rows: dst[(dst_row0 + r) * dst_ld + dst_col0 + c]
+    double *img;            // ident == 0, not null: the rows also go to the panel image of the trailing update
     const double *Lfac;     // factor matrix (the panel's diagonal block is read from it)
     const double *linv_all;
     int ld, dst_ld, nrows, ident;
@@ -284,18 +314,30 @@ __global__ void __launch_bounds__(256) chol_trsm_kernel(const TrsmArgs T)
         const int rr = e >> 8, c = e & 255;
         if (rr < rcount && c < nb) {
             if (T.ident) T.dst[((size_t) blockIdx.y * LNBO + row0 + rr) * LNBO + c] = Xs[rr * TR_LDX + c];
-            else T.dst[(size_t) (row0 + rr) * T.dst_ld + (k0 + c)] = Xs[rr * TR_LDX + c];
+            else {
+                T.dst[(size_t) (row0 + rr) * T.dst_ld + (k0 + c)] = Xs[rr * TR_LDX + c];
+                if (T.img) T.img[syrk_img_index((int) blockIdx.x * TR_ROWS + rr, c)] = Xs[rr * TR_LDX + c];
+            }
         }
     }
 }
 
 // ---- trailing update on the fp64 tensor cores (DMMA) -----------------------------------------------
-// A[r][c] -= sum_{t in [kb,ke)} L[r][t] L[c][t]  for c in [cb,ce), r in [c, nrows).  128x128 CTA
-// tile, 8 warps as 2 (rows) x 4 (cols), warp tile 64x32 = 4x4 m16n8 accumulator tiles of mma.sync.m16n8k8.f64 (the
-// sm_90 shape: four times the work of an m8n8k4 per instruction), K chunks of 16 staged in shared memory with register
-// prefetch of the next chunk.  Both operands are rows of L (A = L, B = L^T), so one fragment pattern serves both:
-// L[row0 + lane/4 (+8)][k + lane%4 (+4)].  The output tile is prefetched into L2 when the CTA starts, so that its
-// read-modify-write at the end does not wait for HBM.
+// A[r][c] -= sum_{t < 256} L[r][t] L[c][t]  for c in [cb, ce), r in [c, nrows), over the 128 x 128 tiles of the lower
+// triangle only.  PERSISTENT: one CTA per SM walks a static list of tiles (column block by column block; CTA b takes tiles
+// b, b + grid, ...), with no atomics and no split K, so the result does not depend on the grid.  WARP-SPECIALISED, 384
+// threads:
+//   warp 8      producer (warps 9..11 only hand their registers to the consumers and leave): a K chunk (32) of one operand of one tile is ONE contiguous 32 KB cp.async.bulk out of the pre-tiled
+//               panel image (below) into a ring of SY_STAGES (A, B) stages with full / empty mbarriers.  It runs ahead across
+//               tiles, so the next tile's first chunks land while the consumers write the previous tile back, and when it
+//               starts on a tile it prefetches that tile's output rows into L2 (the consumers read them a tile later).
+//   warps 0..7  consumers, 2 (rows) x 4 (cols), warp tile 64 x 32 = 4 x 4 accumulators of mma.sync.m16n8k8.f64, fed by
+//               16-byte fragment loads from the stage; inside a chunk the compiler interleaves the loads of the next k8
+//               step with the MMAs of the current one (an explicit register double buffer on top of the 128 accumulator
+//               registers spilled).
+// The arithmetic is that of every earlier version of this update: accumulators start at zero, k ascends in steps of 8 with
+// the same k -> lane mapping, and the tile is written back as C - acc, so the factor does not depend on how the operands
+// reach the tensor cores.
 // D(16x8) += A(16x8) B(8x8); lane = 4 g + t holds A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4], B[t][g], B[t+4][g],
 // D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]
 __device__ __forceinline__ void dmma_m16n8k8(double (&d)[4], const double (&a)[4], const double (&b)[2])
@@ -304,114 +346,156 @@ __device__ __forceinline__ void dmma_m16n8k8(double (&d)[4], const double (&a)[4
                  : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
 }
 
-__global__ void __launch_bounds__(256) chol_syrk_dmma_kernel(double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
+struct SyrkArgs {
+    double *A;              // the matrix being factored (pitch ld, nrows rows)
+    const double *img;      // panel image; its row 0 is matrix row img_row0
+    int ld, nrows, cb, ce, img_row0;
+    int nrb, ntiles;        // row blocks of 128 from cb; lower-triangle tiles of the launch
+};
+
+__global__ void __launch_bounds__(SY_THREADS, 1) chol_syrk_dmma_kernel(const SyrkArgs S)
 {
-    constexpr int BT = 128, BK = 16, LDS = BK + 4;
-    __shared__ double As[BT][LDS];
-    __shared__ double Bs[BT][LDS];
-    const int c0 = cb + blockIdx.x * BT;
-    const int r0 = cb + blockIdx.y * BT;
-    if (r0 + BT <= c0) return;
-    if (c0 >= ce || r0 >= nrows) return;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    using namespace bsfm::ptx;
+    extern __shared__ __align__(128) double ssm[];
+    const uint32_t sbase = smem_u32(ssm);
+    const uint32_t bar_full = sbase + (uint32_t) (SY_STAGES * 2 * SY_BLOCK * sizeof(double)), bar_empty = bar_full + 8 * SY_STAGES;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < SY_STAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, SY_CONSUMERS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const bool vec2 = (S.ld & 1) == 0;      // 16-byte accesses to the output need an even pitch
+    // tile t of the launch -> (row block, column block), column block by column block over the lower triangle
+    auto tile_of = [&](int t, int &rb, int &cbk) {
+        int c = 0;
+        while (t >= S.nrb - c) { t -= S.nrb - c; c++; }
+        cbk = c; rb = c + t;
+    };
+
+    if (warp >= SY_CONSUMERS) {
+        // ===================== producer =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(SY_PRODUCER_REGS));
+        if (warp != SY_CONSUMERS) return;
+        uint64_t keep;      // the panel image is read by a whole column of tiles: keep it in L2
+        asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
+        uint32_t st = 0, ph = 0;
+        for (int t = blockIdx.x; t < S.ntiles; t += gridDim.x) {
+            int rb, cbk;
+            tile_of(t, rb, cbk);
+            const int r0 = S.cb + rb * SY_BT, c0 = S.cb + cbk * SY_BT;
+            const int bytes = (min(SY_BT, S.ce - c0) * 8) & ~15;
+            if (vec2 && bytes > 0)
+                for (int i = lane; i < SY_BT && r0 + i < S.nrows; i += 32) bulk_prefetch_l2(S.A + (size_t) (r0 + i) * S.ld + c0, bytes);
+            if (lane == 0) {
+                const double *ga = S.img + (size_t) ((r0 - S.img_row0) / SY_BT) * SY_KCH * SY_BLOCK;
+                const double *gb = S.img + (size_t) ((c0 - S.img_row0) / SY_BT) * SY_KCH * SY_BLOCK;
+                for (int kc = 0; kc < SY_KCH; kc++) {
+                    mbar_wait_backoff(bar_empty + 8 * st, ph ^ 1);
+                    mbar_expect_tx(bar_full + 8 * st, 2 * SY_BLOCK * sizeof(double));
+                    const uint32_t dst = sbase + st * (uint32_t) (2 * SY_BLOCK * sizeof(double));
+                    tma_bulk_g2s_hint(dst, ga + kc * SY_BLOCK, SY_BLOCK * sizeof(double), bar_full + 8 * st, keep);
+                    tma_bulk_g2s_hint(dst + SY_BLOCK * sizeof(double), gb + kc * SY_BLOCK, SY_BLOCK * sizeof(double), bar_full + 8 * st, keep);
+                    if (++st == SY_STAGES) { st = 0; ph ^= 1; }
+                }
+            }
+            __syncwarp();
+        }
+        return;
+    }
+
+    // ===================== consumers =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(SY_CONSUMER_REGS));
     const int wr = warp >> 2, wc = warp & 3;           // warp tile origin: rows wr*64, cols wc*32
     const int g = lane >> 2, tg = lane & 3;
-    const bool vec2 = (ld & 1) == 0;     // 16-byte accesses need even row pitch
-    if (vec2 && tid < BT && r0 + tid < nrows) {
-        const int bytes = (min(BT, ce - c0) * 8) & ~15;
-        if (bytes > 0)
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(A + (size_t) (r0 + tid) * ld + c0), "r"(bytes) : "memory");
-    }
-    double acc[4][4][4];
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-#pragma unroll
-            for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
-
-    // global -> register prefetch: 128 rows x 16 doubles per operand = 1024 16-byte pieces, 4 per thread
-    double2 pa[4], pb[4];
-    auto fetch = [&](int k0) {
+    // this lane's unit of k8 step s in its rows is 4 tg + (s ^ swz); every fragment row differs from row g by a multiple of 8
+    const int swz = (tg >> 1) ^ ((g & 1) << 1);
+    const double *lane_a = ssm + (wr * 64 + g) * SY_BK + 8 * tg;
+    const double *lane_b = ssm + SY_BLOCK + (wc * 32 + g) * SY_BK + 8 * tg;
+    auto load_frags = [&](double (&af)[4][4], double (&bf)[4][2], uint32_t stage, int s) {
+        const int off = (int) stage * 2 * SY_BLOCK + 2 * (s ^ swz);
 #pragma unroll
         for (int i = 0; i < 4; i++) {
-            const int idx = tid + 256 * i;
-            const int row = idx >> 3, kk = k0 + (idx & 7) * 2;
-            double2 va = make_double2(0.0, 0.0), vb = make_double2(0.0, 0.0);
-            if (r0 + row < nrows) {
-                const double *src = L + (size_t) (r0 + row) * ld + kk;
-                if (kk + 1 < ke) { if (vec2) va = *reinterpret_cast<const double2 *>(src); else { va.x = src[0]; va.y = src[1]; } }
-                else if (kk < ke) va.x = src[0];
-            }
-            if (c0 + row < ce) {
-                const double *src = L + (size_t) (c0 + row) * ld + kk;
-                if (kk + 1 < ke) { if (vec2) vb = *reinterpret_cast<const double2 *>(src); else { vb.x = src[0]; vb.y = src[1]; } }
-                else if (kk < ke) vb.x = src[0];
-            }
-            pa[i] = va; pb[i] = vb;
+            const double2 lo = *reinterpret_cast<const double2 *>(lane_a + off + (i * 16) * SY_BK);
+            const double2 hi = *reinterpret_cast<const double2 *>(lane_a + off + (i * 16 + 8) * SY_BK);
+            af[i][0] = lo.x; af[i][1] = hi.x; af[i][2] = lo.y; af[i][3] = hi.y;
         }
-    };
-    auto stash = [&]() {
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int idx = tid + 256 * i;
-            const int row = idx >> 3, kc = (idx & 7) * 2;
-            *reinterpret_cast<double2 *>(&As[row][kc]) = pa[i];
-            *reinterpret_cast<double2 *>(&Bs[row][kc]) = pb[i];
-        }
-    };
-    fetch(kb);
-    for (int k0 = kb; k0 < ke; k0 += BK) {
-        __syncthreads();
-        stash();
-        __syncthreads();
-        if (k0 + BK < ke) fetch(k0 + BK);
-#pragma unroll
-        for (int ks = 0; ks < BK; ks += 8) {
-            double af[4][4], bf[4][2];
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int r = wr * 64 + i * 16 + g;
-                af[i][0] = As[r][ks + tg]; af[i][1] = As[r + 8][ks + tg];
-                af[i][2] = As[r][ks + tg + 4]; af[i][3] = As[r + 8][ks + tg + 4];
-            }
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const int c = wc * 32 + j * 8 + g;
-                bf[j][0] = Bs[c][ks + tg]; bf[j][1] = Bs[c][ks + tg + 4];
-            }
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < 4; j++) dmma_m16n8k8(acc[i][j], af[i], bf[j]);
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        const int r = r0 + wr * 64 + i * 8 + g;
-        if (r >= nrows) continue;
 #pragma unroll
         for (int j = 0; j < 4; j++) {
-            const int c = c0 + wc * 32 + j * 8 + 2 * tg;
-            const double v0 = acc[i >> 1][j][2 * (i & 1)], v1 = acc[i >> 1][j][2 * (i & 1) + 1];
-            double *dst = A + (size_t) r * ld + c;
-            if (vec2 && c + 1 < ce && c + 1 <= r) {
-                double2 v = *reinterpret_cast<double2 *>(dst);
-                v.x -= v0; v.y -= v1;
-                *reinterpret_cast<double2 *>(dst) = v;
-            } else {
-                if (c < ce && c <= r) dst[0] -= v0;
-                if (c + 1 < ce && c + 1 <= r) dst[1] -= v1;
+            const double2 v = *reinterpret_cast<const double2 *>(lane_b + off + (j * 8) * SY_BK);
+            bf[j][0] = v.x; bf[j][1] = v.y;
+        }
+    };
+    uint32_t st = 0, ph = 0;
+    for (int t = blockIdx.x; t < S.ntiles; t += gridDim.x) {
+        double acc[4][4][4];
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+#pragma unroll
+            for (int j = 0; j < 4; j++)
+#pragma unroll
+                for (int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
+        for (int kc = 0; kc < SY_KCH; kc++) {
+            mbar_wait(bar_full + 8 * st, ph);
+#pragma unroll
+            for (int s = 0; s < 4; s++) {
+                double fa[4][4], fb[4][2];
+                load_frags(fa, fb, st, s);
+#pragma unroll
+                for (int i = 0; i < 4; i++)
+#pragma unroll
+                    for (int j = 0; j < 4; j++) dmma_m16n8k8(acc[i][j], fa[i], fb[j]);
+            }
+            __syncwarp();      // the stage's operands are in registers: hand it back to the producer
+            if (lane == 0) mbar_arrive(bar_empty + 8 * st);
+            if (++st == SY_STAGES) { st = 0; ph ^= 1; }
+        }
+        int rb, cbk;
+        tile_of(t, rb, cbk);
+        const int r0 = S.cb + rb * SY_BT, c0 = S.cb + cbk * SY_BT;
+        // C - acc in four quarters of 16 rows per warp: every load of a quarter is issued before its first store (the compiler
+        // cannot move a load of the matrix past a store to it, so element pair by pair the write-back was 32 serial L2 round
+        // trips; halves instead of quarters spill)
+#pragma unroll
+        for (int h = 0; h < 4; h++) {
+            double2 cur[2][4];
+#pragma unroll
+            for (int pass = 0; pass < 2; pass++) {
+#pragma unroll
+                for (int ii = 0; ii < 2; ii++) {
+                    const int i = 2 * h + ii, r = r0 + wr * 64 + i * 8 + g;
+#pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        const int c = c0 + wc * 32 + j * 8 + 2 * tg;
+                        const bool in0 = r < S.nrows && c < S.ce && c <= r;
+                        const bool in1 = r < S.nrows && c + 1 < S.ce && c + 1 <= r;      // implies in0
+                        double *dst = S.A + (size_t) r * S.ld + c;
+                        if (pass == 0) {      // output read once and written once: stream it through L2
+                            cur[ii][j] = make_double2(0.0, 0.0);
+                            if (vec2 && in1) cur[ii][j] = __ldcs(reinterpret_cast<const double2 *>(dst));
+                            else { if (in0) cur[ii][j].x = dst[0]; if (in1) cur[ii][j].y = dst[1]; }
+                        } else {
+                            const double v0 = cur[ii][j].x - acc[i >> 1][j][2 * (i & 1)], v1 = cur[ii][j].y - acc[i >> 1][j][2 * (i & 1) + 1];
+                            if (vec2 && in1) __stcs(reinterpret_cast<double2 *>(dst), make_double2(v0, v1));
+                            else { if (in0) dst[0] = v0; if (in1) dst[1] = v1; }
+                        }
+                    }
+                }
             }
         }
     }
 }
 
-static void syrk_dmma(cudaStream_t st, double *A, const double *L, int ld, int nrows, int cb, int ce, int kb, int ke)
+// A[r][c] -= L[r][k0 : k0 + 256] . L[c][k0 : k0 + 256] over the lower triangle of rows [cb, nrows) x columns [cb, ce), with
+// the panel read from its image (row 0 = matrix row img_row0 = k0 + 256); at most max_ctas persistent CTAs
+static void syrk_dmma(cudaStream_t st, double *A, const double *img, int ld, int nrows, int cb, int ce, int img_row0, int max_ctas)
 {
-    constexpr int BT = 128;
-    const dim3 grid((ce - cb + BT - 1) / BT, (nrows - cb + BT - 1) / BT);
-    chol_syrk_dmma_kernel<<<grid, 256, 0, st>>>(A, L, ld, nrows, cb, ce, kb, ke);
+    SyrkArgs S = {};
+    S.A = A; S.img = img; S.ld = ld; S.nrows = nrows; S.cb = cb; S.ce = ce; S.img_row0 = img_row0;
+    S.nrb = (nrows - cb + SY_BT - 1) / SY_BT;
+    const int ncb = (ce - cb + SY_BT - 1) / SY_BT;      // <= nrb: ce <= n < nrows
+    S.ntiles = ncb * S.nrb - ncb * (ncb - 1) / 2;
+    chol_syrk_dmma_kernel<<<std::min(S.ntiles, max_ctas), SY_THREADS, SY_SMEM, st>>>(S);
 }
 
 // ---- back substitution L^T x = y, one launch per outer panel (last to first) --------------------------------------
@@ -504,6 +588,7 @@ static int set_smem_attr_once(int dev)
     if (done[dev].load(std::memory_order_acquire)) return BSFM_OK;
     BSFM_CUDA_TRY(cudaFuncSetAttribute(chol_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (DG_SMEM_DOUBLES * sizeof(double))));
     BSFM_CUDA_TRY(cudaFuncSetAttribute(chol_trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (TR_SMEM_DOUBLES * sizeof(double))));
+    BSFM_CUDA_TRY(cudaFuncSetAttribute(chol_syrk_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) SY_SMEM));
     done[dev].store(1, std::memory_order_release);
     return BSFM_OK;
 }
@@ -516,11 +601,21 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
     int dev = 0;
     BSFM_CUDA_TRY(cudaGetDevice(&dev));
     { int rc = set_smem_attr_once(dev); if (rc != BSFM_OK) return rc; }
+    int sms = 0;
+    BSFM_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    // the trailing update reads each panel from its pre-tiled image, kept in xinv_ws until the panel inverses need it
+    double *img = xinv_ws;
+    if (syrk_img_doubles(n) > (size_t) ((n + LNBO - 1) / LNBO) * LNBO * LNBO || (reinterpret_cast<uintptr_t>(img) & 15) != 0) {
+        set_error("chol_solve_large: the panel image does not fit the 16-byte aligned xinv workspace");
+        return BSFM_ERR_ARG;
+    }
     // Look-ahead: the diagonal block of panel p+1 is a serial chain on ONE SM.  The trailing update of panel p is therefore
     // split into the tile columns panel p+1 lives in (launched first) and the rest, and diag(p+1) runs on a side stream next
     // to the rest, taking the first SM the rest's CTAs leave free:
     //   main : trsm(p)  col(p) -E1->  rest(p) ............ -wait E2->  trsm(p+1) ...
     //   side :                 wait E1  diag(p+1) -E2->
+    // The update's CTAs are persistent and hold their SMs to the end, so the rest runs on one SM fewer than the GPU has: that
+    // SM is diag(p+1)'s.
     // BSFM_BA_CHOL_LOOKAHEAD=0 serialises everything on the main stream.
     static const bool lookahead = []() { const char *e = getenv("BSFM_BA_CHOL_LOOKAHEAD"); return !(e && e[0] == '0'); }();
     struct SideStream { int device = -1; cudaStream_t st = nullptr; cudaEvent_t e_col = nullptr, e_diag = nullptr; };
@@ -563,6 +658,7 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
         g_prof.begin(1, st);
         TrsmArgs T = {};
         T.A = A; T.dst = Lmat; T.Lfac = Lmat; T.linv_all = linv_ws; T.ld = ld; T.dst_ld = ld; T.nrows = nrows; T.ident = 0; T.k0 = k0; T.nb = nb; T.n = n;
+        T.img = (k1 < n) ? img : nullptr;      // k1 < n: a full 256-column panel with a trailing update
         chol_trsm_kernel<<<(rows_below + TR_ROWS - 1) / TR_ROWS, 256, TR_SMEM_DOUBLES * sizeof(double), st>>>(T);
         BSFM_KERNEL_CHECK();
         g_prof.end(st);
@@ -574,7 +670,7 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
             }
             const int k2 = std::min(n, k1 + LNBO);      // the columns of panel p+1
             if (lookahead && k2 < n && !tail_fits(k1)) {
-                syrk_dmma(st, A, Lmat, ld, nrows, k1, k2, k0, k1);
+                syrk_dmma(st, A, img, ld, nrows, k1, k2, k1, sms);
                 BSFM_KERNEL_CHECK();
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_col, st));
                 BSFM_CUDA_TRY(cudaStreamWaitEvent(side.st, side.e_col, 0));
@@ -583,9 +679,9 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_diag, side.st));
                 diag_done = true;
                 if (g_prof.on) g_prof.launches[0]++;
-                syrk_dmma(st, A, Lmat, ld, nrows, k2, n, k0, k1);
+                syrk_dmma(st, A, img, ld, nrows, k2, n, k1, sms - 1);
             } else {
-                syrk_dmma(st, A, Lmat, ld, nrows, k1, n, k0, k1);
+                syrk_dmma(st, A, img, ld, nrows, k1, n, k1, sms);
             }
             BSFM_KERNEL_CHECK();
             g_prof.end(st);

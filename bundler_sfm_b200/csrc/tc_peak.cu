@@ -86,14 +86,15 @@ extern "C" double bsfm_measure_int8_peak(int n_tile, int iters)
 }
 
 // ---- fp64 issue rates (dev measurement behind DESIGN.md's notes on the Cholesky pivot chain) ----
-// mode 0: vector DFMA, 8 independent chains per thread;  mode 1: DMMA m8n8k4, 4 independent accumulator pairs per thread.
+// mode 0: vector DFMA, 8 independent chains per thread;  mode 1: DMMA m8n8k4, 4 independent accumulator pairs per thread;
+// mode 2: DMMA m16n8k8 (the Cholesky trailing update's shape), 4 independent accumulator quads per thread.
 // One CTA per SM, `warps` warps; returns SM cycles per warp instruction per SM sub-partition (warps spread over the 4 of them).
 namespace bsfm {
 __global__ void fp64_rate_kernel(int iters, int mode, double *sink, unsigned long long *cycles)
 {
-    double a[8];
+    double a[16];
 #pragma unroll
-    for (int i = 0; i < 8; i++) a[i] = 1.0 + 1e-9 * (threadIdx.x + i);
+    for (int i = 0; i < 16; i++) a[i] = 1.0 + 1e-9 * (threadIdx.x + i);
     const double b = 1.0 + 1e-12 * threadIdx.x, c = 1e-13;
     __syncthreads();
     const unsigned long long t0 = clock64();
@@ -102,17 +103,24 @@ __global__ void fp64_rate_kernel(int iters, int mode, double *sink, unsigned lon
 #pragma unroll
             for (int i = 0; i < 8; i++) a[i] = fma(a[i], b, c);
         }
-    } else {
+    } else if (mode == 1) {
         for (int it = 0; it < iters; it++) {
 #pragma unroll
             for (int i = 0; i < 8; i += 2)
                 asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(a[i]), "+d"(a[i + 1]) : "d"(b), "d"(c));
         }
+    } else {
+        for (int it = 0; it < iters; it++) {
+#pragma unroll
+            for (int i = 0; i < 16; i += 4)
+                asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5, %4, %5}, {%4, %5}, {%0, %1, %2, %3};"
+                             : "+d"(a[i]), "+d"(a[i + 1]), "+d"(a[i + 2]), "+d"(a[i + 3]) : "d"(b), "d"(c));
+        }
     }
     const unsigned long long t1 = clock64();
     double s = 0.0;
 #pragma unroll
-    for (int i = 0; i < 8; i++) s += a[i];
+    for (int i = 0; i < 16; i++) s += a[i];
     if (s == 12345.678) sink[0] = s;
     if (threadIdx.x == 0 && blockIdx.x == 0) cycles[0] = t1 - t0;
 }
@@ -123,7 +131,7 @@ extern "C" double bsfm_measure_fp64_issue_cycles(int mode, int warps, int iters)
     using namespace bsfm;
     clear_error();
     if (require_device() != BSFM_OK) return -1.0;
-    if (warps < 1 || warps > 32 || iters < 16 || (mode != 0 && mode != 1)) { set_error("bsfm_measure_fp64_issue_cycles: bad arguments"); return -1.0; }
+    if (warps < 1 || warps > 32 || iters < 16 || (mode < 0 || mode > 2)) { set_error("bsfm_measure_fp64_issue_cycles: bad arguments"); return -1.0; }
     double *sink = nullptr; unsigned long long *cyc = nullptr, h = 0;
     if (cudaMalloc(&sink, 8) != cudaSuccess || cudaMalloc(&cyc, 8) != cudaSuccess) { set_error("cudaMalloc failed"); return -1.0; }
     fp64_rate_kernel<<<1, 32 * warps>>>(iters, mode, sink, cyc);

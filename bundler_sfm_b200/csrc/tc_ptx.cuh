@@ -1,4 +1,4 @@
-// tc_ptx.cuh -- inline-PTX wrappers of the sm_90a tensor-core kernels (MATCH search, int8 peak loop):
+// tc_ptx.cuh -- inline-PTX wrappers of the sm_90a tensor-core kernels (MATCH search, int8 peak loop, Cholesky trailing update):
 // mbarrier, cp.async.bulk (TMA, also multicast to a cluster), cluster helpers, wgmma.mma_async u8 x u8 -> s32 and its
 // shared-memory descriptors.
 #pragma once
@@ -56,7 +56,19 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void *src, uint
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-// the same, delivered to the same shared-memory offset in every CTA of `cta_mask` (cluster), completing on the mbarrier at the
+// the same with an L2 cache policy (createpolicy) for the source
+__device__ __forceinline__ void tma_bulk_g2s_hint(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar, uint64_t policy)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(policy) : "memory");
+}
+// bring `bytes` (multiple of 16, 16-byte aligned source) into L2 without waiting for them
+__device__ __forceinline__ void bulk_prefetch_l2(const void *src, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
+
+// tma_bulk_g2s, delivered to the same shared-memory offset in every CTA of `cta_mask` (cluster), completing on the mbarrier at the
 // same offset in each of them
 __device__ __forceinline__ void tma_bulk_g2s_multicast(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar, uint16_t cta_mask)
 {

@@ -38,8 +38,10 @@ int bsfm_set_device(int device);
  * bench.py uses it as the denominator of the tensor rooflines (SURVEY.md 8d).  < 0 on error.                        */
 double bsfm_measure_int8_peak(int n_tile, int iters);
 /* Measured fp64 issue interval of the current device: SM cycles per warp instruction per SM sub-partition with `warps` resident
- * warps of one CTA; mode 0 = vector DFMA (8 independent chains per thread), mode 1 = DMMA m8n8k4 (4 independent accumulators).
- * The numbers behind DESIGN.md's notes on the Cholesky pivot chain (csrc/tc_peak.cu).  < 0 on error.                */
+ * warps of one CTA; mode 0 = vector DFMA (8 independent chains per thread), mode 1 = DMMA m8n8k4 (4 independent accumulators),
+ * mode 2 = DMMA m16n8k8 (4 independent accumulators; the shape of the large Cholesky's trailing update, 2048 fp64 FLOP per
+ * instruction, so 2048 * 4 / cycles is the SM's fp64 tensor rate in FLOP per clock).  The numbers behind DESIGN.md's notes
+ * on the Cholesky (csrc/tc_peak.cu).  < 0 on error.                                                              */
 double bsfm_measure_fp64_issue_cycles(int mode, int warps, int iters);
 /* number of CUDA devices visible to this process (0 when there is none) */
 int bsfm_device_count(void);
