@@ -29,7 +29,9 @@ class CameraParams(ctypes.Structure):
     ]
 
 
-def make_cameras(R, c, f, k, constrained=None, constraints=None, weights=None):
+def make_cameras(R, c, f, k, constrained=None, constraints=None, weights=None, known=None, K_known=None, k_known=None):
+    """camera_params_t array.  known (m flags), K_known (m x 9) and k_known (m x 5) describe calibrated cameras
+    (known_intrinsics, lib/sfm-driver/sfm.c:339-357); without them every camera is an ordinary one."""
     m = len(f)
     cams = (CameraParams * m)()
     for j in range(m):
@@ -44,6 +46,10 @@ def make_cameras(R, c, f, k, constrained=None, constraints=None, weights=None):
                            bytes(bytearray(int(v) for v in constrained[j])), NUM_CAMERA_PARAMS)
             cams[j].constraints[:] = list(np.asarray(constraints[j], float))
             cams[j].weights[:] = list(np.asarray(weights[j], float))
+        if known is not None and known[j]:
+            cams[j].known_intrinsics = b"\x01"
+            cams[j].K_known[:] = list(np.asarray(K_known[j], float).reshape(9))
+            cams[j].k_known[:] = list(np.asarray(k_known[j], float).reshape(5))
     return cams
 
 
@@ -67,13 +73,14 @@ def _bind_run_sfm(fn):
 def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_centers=1, ncons=0, eps2=1e-12,
                  use_constraints=0, constrained=None, constraints=None, weights=None,
                  use_point_constraints=0, points_constraints=None, point_constraint_weight=0.0,
-                 extra_info=False, export=False, fix_points=0):
+                 extra_info=False, export=False, fix_points=0, known=None, K_known=None, k_known=None):
     """Calls a run_sfm-shaped C function (ours or the reference's) on a scene dict (synth.ba_scene).
+    known / K_known / k_known: calibrated cameras (see make_cameras).
     Returns a dict with the refined R, c, f, k, pts (+ info when the callee provides it)."""
     vmask = np.ascontiguousarray(scene["vmask"], dtype=np.int8)
     n, m = vmask.shape
     proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
-    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], constrained, constraints, weights)
+    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], constrained, constraints, weights, known, K_known, k_known)
     pts = np.ascontiguousarray(scene["pts"], dtype=np.float64).copy()
     pc = None
     if use_point_constraints:
@@ -101,7 +108,8 @@ _run_sfm = None
 
 
 def run_sfm(scene, **kw):
-    """GPU run_sfm (bsfm_run_sfm).  Raises on BSFM errors; returns the refined scene + info[10]."""
+    """GPU run_sfm (bsfm_run_sfm).  Raises on BSFM errors; returns the refined scene + info[10].
+    Keywords are those of call_run_sfm (known / K_known / k_known for calibrated cameras)."""
     global _run_sfm
     lib = load_library()
     if _run_sfm is None:
@@ -127,15 +135,35 @@ def last_timing():
     return d
 
 
-def reprojection_rmse(scene, sol):
+def project_known(Pc, K_known, k_known):
+    """the calibrated-camera branch of sfm_project_rd (lib/sfm-driver/sfm.c:339-357) on camera-frame points Pc (N x 3)
+    with per-point K_known (N x 9) and k_known (N x 5), in the reference's operation order -> pixels (N x 2)"""
+    x_n = -Pc[:, 0] / Pc[:, 2]
+    y_n = -Pc[:, 1] / Pc[:, 2]
+    k, K = k_known, K_known
+    rsq = x_n * x_n + y_n * y_n
+    factor = 1.0 + k[:, 0] * rsq + k[:, 1] * rsq * rsq + k[:, 4] * rsq * rsq * rsq
+    dx_x = 2 * k[:, 2] * x_n * y_n + k[:, 3] * (rsq + 2 * x_n * x_n)
+    dx_y = k[:, 2] * (rsq + 2 * y_n * y_n) + 2 * k[:, 3] * x_n * y_n
+    x_d = x_n * factor + dx_x
+    y_d = y_n * factor + dx_y
+    return np.stack([K[:, 0] * x_d + K[:, 1] * y_d + K[:, 2], K[:, 4] * y_d + K[:, 5]], 1)
+
+
+def reprojection_rmse(scene, sol, known=None, K_known=None, k_known=None):
     """sqrt(mean squared reprojection error) of a solution under the Bundler camera model
-    (lib/sfm-driver/sfm.c:302-380), computed in numpy -- a test/bench metric, not a product path."""
+    (lib/sfm-driver/sfm.c:302-380), computed in numpy -- a test/bench metric, not a product path.
+    known / K_known / k_known: calibrated cameras, as for run_sfm."""
     vmask = scene["vmask"]
     pi, cj = np.nonzero(vmask)
     R = sol["R"].reshape(-1, 3, 3)
     Pc = np.einsum("oij,oj->oi", R[cj], sol["pts"][pi] - sol["c"][cj])
     f = sol["f"][cj]
     p = -Pc[:, :2] * f[:, None] / Pc[:, 2:3]
+    if known is not None:
+        kn = np.asarray(known, bool)[cj]
+        if kn.any():
+            p[kn] = project_known(Pc[kn], np.asarray(K_known, float).reshape(-1, 9)[cj[kn]], np.asarray(k_known, float)[cj[kn]])
     rsq = (p ** 2).sum(1) / (f * f)
     k = sol["k"][cj]
     p = p * (1.0 + k[:, 0] * rsq + k[:, 1] * rsq * rsq)[:, None]
@@ -202,33 +230,66 @@ def unpack_params(p, scene, est_focal_length=1, undistort=1, f_scale=0.001, k_sc
 
 
 def levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, cnp, R_init, f_fixed, est_focal_length=1, undistort=1,
-                 explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, eps5=4.0e-2):
+                 explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, eps5=4.0e-2, init_params=None):
     """bsfm_sba_motstr_levmar_model with raw (host or DEVICE) pointers for vmask / p / x.
+    init_params: a make_cameras array whose calibrated cameras the projection uses (bsfm_sba_motstr_levmar_model_ki).
     Returns (iterations, info[10])."""
     lib = load_library()
-    fn = lib.bsfm_sba_motstr_levmar_model
+    name = "bsfm_sba_motstr_levmar_model" if init_params is None else "bsfm_sba_motstr_levmar_model_ki"
+    fn = getattr(lib, name)
     c = ctypes
     fn.argtypes = [c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int,
                    c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p, c.c_int, c.c_void_p,
-                   c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p]
+                   c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p] + ([] if init_params is None else [c.c_void_p])
     fn.restype = c.c_int
     R_init = np.ascontiguousarray(R_init, dtype=np.float64)
     f_fixed = np.ascontiguousarray(f_fixed, dtype=np.float64)
     model = SfmModel(est_focal_length, undistort, explicit_camera_centers, 0.001, 5.0, R_init.ctypes.data, f_fixed.ctypes.data)
     opts = np.array([1.0e-3, 1.0e-10, eps2, 1.0e-12, 0.0, eps5])     # sfm.c:705-714 (opts[5] = 4e-2 there)
     info = np.zeros(10)
-    rc = fn(n, m, 0, vmask_ptr, p_ptr, cnp, 3, x_ptr, None, 2, ctypes.addressof(model), jac_mode, itmax, verbose,
-            opts.ctypes.data, info.ctypes.data, 0, None, 0, None, None, None, None, None)
+    args = [n, m, 0, vmask_ptr, p_ptr, cnp, 3, x_ptr, None, 2, ctypes.addressof(model), jac_mode, itmax, verbose,
+            opts.ctypes.data, info.ctypes.data, 0, None, 0, None, None, None, None, None]
+    if init_params is not None:
+        args.append(ctypes.addressof(init_params))
+    rc = fn(*args)
     if rc < -1:
-        check(rc, "bsfm_sba_motstr_levmar_model")
+        check(rc, name)
     return rc, info
 
 
-def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thresh=16.0, pt_protected=None, cap=None):
+def mot_levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, points_ptr, cnp, R_init, f_fixed, est_focal_length=1, undistort=1,
+                     explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, init_params=None):
+    """motion-only counterpart of levmar_model: bsfm_sba_mot_levmar_model(_ki) with raw (host or DEVICE) pointers for
+    vmask / p (cameras only) / x / points (n x 3, fixed).  Returns (iterations, info[10])."""
+    lib = load_library()
+    name = "bsfm_sba_mot_levmar_model" if init_params is None else "bsfm_sba_mot_levmar_model_ki"
+    fn = getattr(lib, name)
+    c = ctypes
+    fn.argtypes = [c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p, c.c_void_p, c.c_int,
+                   c.c_void_p, c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p] + \
+        ([] if init_params is None else [c.c_void_p])
+    fn.restype = c.c_int
+    R_init = np.ascontiguousarray(R_init, dtype=np.float64)
+    f_fixed = np.ascontiguousarray(f_fixed, dtype=np.float64)
+    model = SfmModel(est_focal_length, undistort, explicit_camera_centers, 0.001, 5.0, R_init.ctypes.data, f_fixed.ctypes.data)
+    opts = np.array([1.0e-3, 1.0e-10, eps2, 1.0e-12, 0.0, 4.0e-2])
+    info = np.zeros(10)
+    args = [n, m, 0, vmask_ptr, p_ptr, cnp, x_ptr, None, 2, ctypes.addressof(model), points_ptr, jac_mode, itmax, verbose,
+            opts.ctypes.data, info.ctypes.data, 0, None]
+    if init_params is not None:
+        args.append(ctypes.addressof(init_params))
+    rc = fn(*args)
+    if rc < -1:
+        check(rc, name)
+    return rc, info
+
+
+def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thresh=16.0, pt_protected=None, cap=None,
+                          known=None, K_known=None, k_known=None):
     """bsfm_reprojection_outliers: the statistics / outlier pass BundlerApp::RunSFM_SBA runs after every run_sfm
     (src/Bundle.cpp:659-856) on a scene dict (vmask, projections, R, c, f, k, pts).  Defaults are bundler's
     m_min/max_proj_error_threshold (BundlerApp.h).  Returns dist[nvis], stats[m x 5] (n, mean, median, med80, thresh),
-    outliers, errors, global_mean."""
+    outliers, errors, global_mean.  known / K_known / k_known: calibrated cameras, as for run_sfm."""
     lib = load_library()
     fn = lib.bsfm_reprojection_outliers
     fn.restype = ctypes.c_int
@@ -238,7 +299,7 @@ def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thre
     vmask = np.ascontiguousarray(scene["vmask"], dtype=np.int8)
     n, m = vmask.shape
     proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
-    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"])
+    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], known=known, K_known=K_known, k_known=k_known)
     pts = np.ascontiguousarray(scene["pts"], dtype=np.float64)
     prot = None if pt_protected is None else np.ascontiguousarray(pt_protected, dtype=np.int8)
     nvis = proj.shape[0]

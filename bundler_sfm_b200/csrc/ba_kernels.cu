@@ -120,9 +120,12 @@ __device__ __forceinline__ double fd_step(double v)
     return d;
 }
 
-// sfm_project_point3 + sfm_project_rd (lib/sfm-driver/sfm.c:503-552, 302-380), known_intrinsics = 0
-__device__ __forceinline__ void project_dev(const Model &M, const double (&a)[MAX_CNP], const double *R, double f_fixed,
-                                            double b0, double b1, double b2, double &px, double &py)
+// sfm_project_point3 + sfm_project_rd (lib/sfm-driver/sfm.c:503-552, 302-380).  KI = false: every camera takes the
+// known_intrinsics = 0 branch and `ci` is not read.  KI = true: calibrated cameras (ci->known) take the other branch;
+// the radial step after it is the same for both and still uses the focal parameter K0.
+template <bool KI>
+__device__ __forceinline__ void project_dev(const Model &M, const CamIntrinsics *ci, const double (&a)[MAX_CNP], const double *R,
+                                            double f_fixed, double b0, double b1, double b2, double &px, double &py)
 {
     double bc0, bc1, bc2;
     if (M.explicit_centers) {
@@ -137,8 +140,13 @@ __device__ __forceinline__ void project_dev(const Model &M, const double (&a)[MA
         bc0 += a[0]; bc1 += a[1]; bc2 += a[2];
     }
     const double K0 = M.est_focal ? a[6] / M.f_scale : f_fixed;
-    double p0 = -bc0 * K0 / bc2;
-    double p1 = -bc1 * K0 / bc2;
+    double p0, p1;
+    if (KI && ci->known) {
+        project_known_dev(*ci, bc0, bc1, bc2, p0, p1);
+    } else {
+        p0 = -bc0 * K0 / bc2;
+        p1 = -bc1 * K0 / bc2;
+    }
     if (M.undistort) {
         const double k1 = (M.est_focal ? a[7] : a[6]) / M.k_scale;
         const double k2 = (M.est_focal ? a[8] : a[7]) / M.k_scale;
@@ -186,6 +194,7 @@ __global__ void cam_prep_kernel(Problem P, const double *p, int with_pert)
 // K1: e = x - f(p), sum e^2 (sba_levmar.c:802-806, nrmL2xmy :159-207)
 // also: stop-8 statistic against a previous residual vector when e_prev != nullptr (:1552-1561)
 // ------------------------------------------------------------------------------------------------
+template <bool KI>
 __global__ void residual_kernel(Problem P, const double *p, double *e_out, const double *e_prev, double eps5)
 {
     cudaGridDependencySynchronize();   // programmatic dependent launch (see launch_pdl)
@@ -197,7 +206,7 @@ __global__ void residual_kernel(Problem P, const double *p, double *e_out, const
         load_cam(P, p, j, a);
         const double *b = p + (size_t) P.m * P.M.cnp + (size_t) i * 3;
         double hx, hy;
-        project_dev(P.M, a, P.camR + (size_t) j * 36, P.f_fixed[j], b[0], b[1], b[2], hx, hy);
+        project_dev<KI>(P.M, KI ? P.intr + j : nullptr, a, P.camR + (size_t) j * 36, P.f_fixed[j], b[0], b[1], b[2], hx, hy);
         const double e0 = P.x[2 * (size_t) o] - hx, e1 = P.x[2 * (size_t) o + 1] - hy;
         e_out[2 * (size_t) o] = e0;
         e_out[2 * (size_t) o + 1] = e1;
@@ -218,12 +227,15 @@ __global__ void residual_kernel(Problem P, const double *p, double *e_out, const
         if (grid_reduce<1>(pct, P.partial + gridDim.x, P.ticket + 1, out)) P.sc->max_pct = out;
     }
 }
+template __global__ void residual_kernel<false>(Problem, const double *, double *, const double *, double);
+template __global__ void residual_kernel<true>(Problem, const double *, double *, const double *, double);
 
 // ------------------------------------------------------------------------------------------------
 // K2 + W of K3: per observation A_ij (2 x cnp), B_ij (2 x 3), W_ij = A^T B (cnp x 3)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void analytic_jac(const Problem &P, const double (&a)[MAX_CNP], const double *R0, double f_fixed,
-                                             double b0, double b1, double b2, double (&A)[2][MAX_CNP], double (&B)[2][3])
+template <bool KI>
+__device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsics *ci, const double (&a)[MAX_CNP], const double *R0,
+                                             double f_fixed, double b0, double b1, double b2, double (&A)[2][MAX_CNP], double (&B)[2][3])
 {
     // SURVEY.md A.4.  v = R_init (X - c) [or R_init X], Pc = exp([w]x) v (+ t), q = -Pc.xy / Pc.z
     const Model &M = P.M;
@@ -243,16 +255,54 @@ __device__ __forceinline__ void analytic_jac(const Problem &P, const double (&a)
     const double k2 = M.undistort ? (M.est_focal ? a[8] : a[7]) / M.k_scale : 0.0;
     const double iz = 1.0 / Pc2;
     const double q0 = -Pc0 * iz, q1 = -Pc1 * iz;
-    const double rho = q0 * q0 + q1 * q1;
-    const double r = 1.0 + k1 * rho + k2 * rho * rho;
-    const double g = 2.0 * (k1 + 2.0 * k2 * rho);
-    // dxhat/dq (2x2) = f ( r I + g q q^T )
-    const double D00 = f * (r + g * q0 * q0), D01 = f * g * q0 * q1, D11 = f * (r + g * q1 * q1);
-    // dq/dPc (2x3) = -(1/z) [ I | q ]
-    // G = dxhat/dPc (2x3)
     double G[2][3];
-    G[0][0] = -iz * D00; G[0][1] = -iz * D01; G[0][2] = -iz * (D00 * q0 + D01 * q1);
-    G[1][0] = -iz * D01; G[1][1] = -iz * D11; G[1][2] = -iz * (D01 * q0 + D11 * q1);
+    double Ai[2][3];   // calibrated camera: columns of f*f_scale, k1*k_scale, k2*k_scale (sfm.c:673-681)
+    double rho, r;
+    if (KI && ci->known) {
+        // calibrated camera: u = Kc d(q) (Brown-Conrady d, Kc = [[K0, K1], [0, K4]]), then the radial step
+        // xhat = u (1 + k1 s + k2 s^2), s = |u|^2 / f^2.  dxhat/dq = (fac I + h u u^T) Kc Jd, h = 2 (k1 + 2 k2 s) / f^2
+        const double *kd = ci->k, *Kc = ci->K;
+        const double rsq = q0 * q0 + q1 * q1;
+        const double F = 1.0 + kd[0] * rsq + kd[1] * rsq * rsq + kd[4] * rsq * rsq * rsq;
+        const double dF = kd[0] + 2.0 * kd[1] * rsq + 3.0 * kd[4] * rsq * rsq;
+        const double xd = q0 * F + 2.0 * kd[2] * q0 * q1 + kd[3] * (rsq + 2.0 * q0 * q0);
+        const double yd = q1 * F + kd[2] * (rsq + 2.0 * q1 * q1) + 2.0 * kd[3] * q0 * q1;
+        // Jd = d(xd, yd)/d(q0, q1) (symmetric)
+        const double J00 = F + 2.0 * q0 * q0 * dF + 2.0 * kd[2] * q1 + 6.0 * kd[3] * q0;
+        const double J01 = 2.0 * q0 * q1 * dF + 2.0 * kd[2] * q0 + 2.0 * kd[3] * q1;
+        const double J11 = F + 2.0 * q1 * q1 * dF + 6.0 * kd[2] * q1 + 2.0 * kd[3] * q0;
+        const double M00 = Kc[0] * J00 + Kc[1] * J01, M01 = Kc[0] * J01 + Kc[1] * J11;
+        const double M10 = Kc[3] * J01, M11 = Kc[3] * J11;
+        const double u0 = Kc[0] * xd + Kc[1] * yd + Kc[2], u1 = Kc[3] * yd + Kc[4];
+        // without the radial step f is not read at all (it may be unset when it is not estimated either)
+        const double s = M.undistort ? (u0 * u0 + u1 * u1) / (f * f) : 0.0;
+        const double fac = 1.0 + k1 * s + k2 * s * s;
+        const double h = M.undistort ? 2.0 * (k1 + 2.0 * k2 * s) / (f * f) : 0.0;
+        const double P00 = fac + h * u0 * u0, P01 = h * u0 * u1, P11 = fac + h * u1 * u1;
+        const double D00 = P00 * M00 + P01 * M10, D01 = P00 * M01 + P01 * M11;
+        const double D10 = P01 * M00 + P11 * M10, D11 = P01 * M01 + P11 * M11;
+        G[0][0] = -iz * D00; G[0][1] = -iz * D01; G[0][2] = -iz * (D00 * q0 + D01 * q1);
+        G[1][0] = -iz * D10; G[1][1] = -iz * D11; G[1][2] = -iz * (D10 * q0 + D11 * q1);
+        // the focal length enters only through s (zero column without the radial step)
+        const double dsf = M.undistort ? -2.0 * s / f * (k1 + 2.0 * k2 * s) : 0.0;
+        const double uu[2] = {u0, u1};
+#pragma unroll
+        for (int k = 0; k < 2; k++) {
+            Ai[k][0] = uu[k] * dsf / M.f_scale;
+            Ai[k][1] = uu[k] * s / M.k_scale;
+            Ai[k][2] = uu[k] * s * s / M.k_scale;
+        }
+    } else {
+        rho = q0 * q0 + q1 * q1;
+        r = 1.0 + k1 * rho + k2 * rho * rho;
+        const double g = 2.0 * (k1 + 2.0 * k2 * rho);
+        // dxhat/dq (2x2) = f ( r I + g q q^T )
+        const double D00 = f * (r + g * q0 * q0), D01 = f * g * q0 * q1, D11 = f * (r + g * q1 * q1);
+        // dq/dPc (2x3) = -(1/z) [ I | q ]
+        // G = dxhat/dPc (2x3)
+        G[0][0] = -iz * D00; G[0][1] = -iz * D01; G[0][2] = -iz * (D00 * q0 + D01 * q1);
+        G[1][0] = -iz * D01; G[1][1] = -iz * D11; G[1][2] = -iz * (D01 * q0 + D11 * q1);
+    }
     // B = G R ; dPc/dc = -R (explicit centres) or dPc/dt = I
 #pragma unroll
     for (int k = 0; k < 2; k++)
@@ -290,15 +340,17 @@ __device__ __forceinline__ void analytic_jac(const Problem &P, const double (&a)
     const double qq[2] = {q0, q1};
 #pragma unroll
     for (int k = 0; k < 2; k++) {
-        const double dfs = r * qq[k] / M.f_scale;
-        const double dk1 = f * rho * qq[k] / M.k_scale;
-        const double dk2 = f * rho * rho * qq[k] / M.k_scale;
+        const bool kn = KI && ci->known;
+        const double dfs = kn ? Ai[k][0] : r * qq[k] / M.f_scale;
+        const double dk1 = kn ? Ai[k][1] : f * rho * qq[k] / M.k_scale;
+        const double dk2 = kn ? Ai[k][2] : f * rho * rho * qq[k] / M.k_scale;
         A[k][6] = M.est_focal ? dfs : (M.undistort ? dk1 : 0.0);
         A[k][7] = M.est_focal ? (M.undistort ? dk1 : 0.0) : (M.undistort ? dk2 : 0.0);
         A[k][8] = (M.est_focal && M.undistort) ? dk2 : 0.0;
     }
 }
 
+template <bool KI>
 __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *p, int jac_mode)
 {
     cudaGridDependencySynchronize();   // programmatic dependent launch (see launch_pdl)
@@ -312,14 +364,15 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
     const double *bp = p + (size_t) P.m * cnp + (size_t) i * 3;
     double b[3] = {bp[0], bp[1], bp[2]};
     const double ff = P.f_fixed[j];
+    const CamIntrinsics *ci = KI ? P.intr + j : nullptr;
     double A[2][MAX_CNP], B[2][3];
 
     if (jac_mode == 1) {
-        analytic_jac(P, a, P.R_init + (size_t) j * 9, ff, b[0], b[1], b[2], A, B);
+        analytic_jac<KI>(P, ci, a, P.R_init + (size_t) j * 9, ff, b[0], b[1], b[2], A, B);
     } else {
         const double *Rb = P.camR + (size_t) j * 36;
         double h0, h1;
-        project_dev(M, a, Rb, ff, b[0], b[1], b[2], h0, h1);
+        project_dev<KI>(M, ci, a, Rb, ff, b[0], b[1], b[2], h0, h1);
 #pragma unroll
         for (int jj = 0; jj < MAX_CNP; jj++) {
             A[0][jj] = 0.0; A[1][jj] = 0.0;
@@ -330,7 +383,7 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
                 a[jj] = tmp + d;
                 const double *R = (jj >= 3 && jj <= 5) ? (Rb + 9 * (jj - 2)) : Rb;
                 double g0, g1;
-                project_dev(M, a, R, ff, b[0], b[1], b[2], g0, g1);
+                project_dev<KI>(M, ci, a, R, ff, b[0], b[1], b[2], g0, g1);
                 a[jj] = tmp;
                 A[0][jj] = (g0 - h0) * d1;
                 A[1][jj] = (g1 - h1) * d1;
@@ -343,7 +396,7 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
             const double tmp = b[jj];
             b[jj] = tmp + d;
             double g0, g1;
-            project_dev(M, a, Rb, ff, b[0], b[1], b[2], g0, g1);
+            project_dev<KI>(M, ci, a, Rb, ff, b[0], b[1], b[2], g0, g1);
             b[jj] = tmp;
             B[0][jj] = (g0 - h0) * d1;
             B[1][jj] = (g1 - h1) * d1;
@@ -370,6 +423,8 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
 #pragma unroll
     for (int jj = 0; jj < 3; jj++) { jB[jj] = B[0][jj]; jB[3 + jj] = B[1][jj]; }
 }
+template __global__ void jacobian_kernel<false>(Problem, const double *, int);
+template __global__ void jacobian_kernel<true>(Problem, const double *, int);
 
 // ------------------------------------------------------------------------------------------------
 // K3: V_i, eb_i -- one thread per point, observations in ascending camera order (same summation

@@ -7,6 +7,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include "../../include/bsfm_b200_ba.h"
 
 namespace bsfm {
 namespace ba {
@@ -23,6 +24,44 @@ struct Model {
     int k_idx;       // 7, 6 or -1
     double f_scale, k_scale;
 };
+
+// Calibrated camera (camera_params_t::known_intrinsics, K_known, k_known; lib/sfm-driver/sfm.c:339-357): a full
+// upper-triangular K and five Brown-Conrady coefficients replace the focal-only pinhole before the radial step.
+// Uploaded once per solve, and only when some camera is calibrated.
+struct CamIntrinsics {
+    double K[5];    // K_known[0], [1], [2], [4], [5] (the reference never reads K_known[3] or [6..8])
+    double k[5];    // k_known[0..4]: radial k0, k1, tangential k2, k3, radial k4
+    int known;      // known_intrinsics != 0
+    int pad;
+};
+
+// the table entry of one camera_params_t (host side; solver and outlier pass)
+inline CamIntrinsics cam_intrinsics(const bsfm_camera_params_t &c)
+{
+    CamIntrinsics ci;
+    ci.K[0] = c.K_known[0]; ci.K[1] = c.K_known[1]; ci.K[2] = c.K_known[2]; ci.K[3] = c.K_known[4]; ci.K[4] = c.K_known[5];
+    for (int q = 0; q < 5; q++) ci.k[q] = c.k_known[q];
+    ci.known = c.known_intrinsics ? 1 : 0;
+    ci.pad = 0;
+    return ci;
+}
+
+// Brown-Conrady distortion and K of a calibrated camera (the known_intrinsics branch of sfm_project_rd,
+// lib/sfm-driver/sfm.c:339-357), in the reference's operation order
+__device__ __forceinline__ void project_known_dev(const CamIntrinsics &ci, double bc0, double bc1, double bc2, double &p0, double &p1)
+{
+    const double x_n = -bc0 / bc2;
+    const double y_n = -bc1 / bc2;
+    const double *k = ci.k;
+    const double rsq = x_n * x_n + y_n * y_n;
+    const double factor = 1.0 + k[0] * rsq + k[1] * rsq * rsq + k[4] * rsq * rsq * rsq;
+    const double dx_x = 2.0 * k[2] * x_n * y_n + k[3] * (rsq + 2.0 * x_n * x_n);
+    const double dx_y = k[2] * (rsq + 2.0 * y_n * y_n) + 2.0 * k[3] * x_n * y_n;
+    const double x_d = x_n * factor + dx_x;
+    const double y_d = y_n * factor + dx_y;
+    p0 = ci.K[0] * x_d + ci.K[1] * y_d + ci.K[2];
+    p1 = ci.K[3] * y_d + ci.K[4];
+}
 
 // scalars produced on the device, copied to pinned host memory once per LM phase
 struct Scalars {
@@ -86,6 +125,7 @@ struct Problem {
     unsigned int *ticket;  // last-block counters
     Scalars *sc;      // device scalars
     const double *mu; // damping term of the current try (device scalar, written by the host)
+    const CamIntrinsics *intr;  // m entries, or null when no camera is calibrated (then only the KI = false kernels run)
 };
 
 // launch with the programmatic-stream-serialization attribute (PDL): the launch latency of a kernel overlaps

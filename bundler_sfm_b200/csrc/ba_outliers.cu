@@ -16,6 +16,7 @@
 #include <cub/cub.cuh>
 
 #include "common.h"
+#include "ba_kernels.cuh"
 #include "../../include/bsfm_b200_ba.h"
 
 namespace bsfm {
@@ -26,9 +27,11 @@ __global__ void vmask_fill_kernel(const char *, int, int, const int *, int *, in
 
 struct CamCompact { double R[9], t[3], f, k0, k1; };
 
-// one thread per observation (point-major order == the order of `projections`)
-__global__ void outlier_dist_kernel(int nvis, const int *obs_cam, const int *obs_pt, const CamCompact *cams, const double *pts,
-                                    const double *proj, int undistort, double *dist)
+// one thread per observation (point-major order == the order of `projections`).  KI: `intr` (m entries) holds the
+// calibrated cameras; KI = false never reads it.
+template <bool KI>
+__global__ void outlier_dist_kernel(int nvis, const int *obs_cam, const int *obs_pt, const CamCompact *cams, const CamIntrinsics *intr,
+                                    const double *pts, const double *proj, int undistort, double *dist)
 {
     const int o = blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= nvis) return;
@@ -39,8 +42,13 @@ __global__ void outlier_dist_kernel(int nvis, const int *obs_cam, const int *obs
     const double c0 = C.R[0] * b0 + C.R[1] * b1 + C.R[2] * b2;
     const double c1 = C.R[3] * b0 + C.R[4] * b1 + C.R[5] * b2;
     const double c2 = C.R[6] * b0 + C.R[7] * b1 + C.R[8] * b2;
-    double p0 = -c0 * C.f / c2;
-    double p1 = -c1 * C.f / c2;
+    double p0, p1;
+    if (KI && intr[obs_cam[o]].known) {
+        project_known_dev(intr[obs_cam[o]], c0, c1, c2, p0, p1);
+    } else {
+        p0 = -c0 * C.f / c2;
+        p1 = -c1 * C.f / c2;
+    }
     if (undistort) {   // sfm.c:362-377
         const double rsq = (p0 * p0 + p1 * p1) / (C.f * C.f);
         const double factor = 1.0 + C.k0 * rsq + C.k1 * rsq * rsq;
@@ -145,8 +153,11 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
         set_error("bsfm_reprojection_outliers: bad arguments");
         return BSFM_ERR_ARG;
     }
-    for (int j = 0; j < m; j++)
-        if (cams[j].known_intrinsics || cams[j].fisheye) { set_error("bsfm_reprojection_outliers: known_intrinsics / fisheye cameras are outside the GPU path"); return BSFM_ERR_UNSUPPORTED; }
+    bool any_known = false;
+    for (int j = 0; j < m; j++) {
+        if (cams[j].fisheye) { set_error("bsfm_reprojection_outliers: fisheye cameras are outside the GPU path"); return BSFM_ERR_UNSUPPORTED; }
+        any_known = any_known || cams[j].known_intrinsics;
+    }
 
     DevBuf D;
     char *d_vmask, *d_prot = nullptr;
@@ -194,6 +205,13 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
     BSFM_CUDA_TRY(D.alloc(&d_iota, (size_t) nvis)); BSFM_CUDA_TRY(D.alloc(&d_cam_obs, (size_t) nvis)); BSFM_CUDA_TRY(D.alloc(&d_cam_sorted, (size_t) nvis));
     BSFM_CUDA_TRY(D.alloc(&d_cam_ptr, (size_t) m + 1)); BSFM_CUDA_TRY(D.alloc(&d_first, (size_t) n));
     BSFM_CUDA_TRY(cudaMemcpy(d_cams, hc.data(), (size_t) m * sizeof(CamCompact), cudaMemcpyHostToDevice));
+    CamIntrinsics *d_intr = nullptr;     // calibrated cameras (sfm.c:339-357): side table, only when there is one
+    if (any_known) {
+        std::vector<CamIntrinsics> hi(m);
+        for (int j = 0; j < m; j++) hi[j] = cam_intrinsics(cams[j]);
+        BSFM_CUDA_TRY(D.alloc(&d_intr, (size_t) m));
+        BSFM_CUDA_TRY(cudaMemcpy(d_intr, hi.data(), (size_t) m * sizeof(CamIntrinsics), cudaMemcpyHostToDevice));
+    }
     BSFM_CUDA_TRY(cudaMemcpy(d_pts, pts, (size_t) n * 3 * sizeof(double), cudaMemcpyDefault));
     BSFM_CUDA_TRY(cudaMemcpy(d_proj, projections, (size_t) nvis * 2 * sizeof(double), cudaMemcpyDefault));
     if (pt_protected) {
@@ -201,7 +219,8 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
         BSFM_CUDA_TRY(cudaMemcpy(d_prot, pt_protected, (size_t) n, cudaMemcpyDefault));
     }
     const int gb = (nvis + 255) / 256;
-    outlier_dist_kernel<<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
+    if (d_intr) outlier_dist_kernel<true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
+    else outlier_dist_kernel<false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
     BSFM_KERNEL_CHECK();
 
     // camera-major view (stable sort by camera keeps ascending point order), per-camera sorted distances

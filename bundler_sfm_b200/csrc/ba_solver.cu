@@ -25,8 +25,8 @@
 namespace bsfm {
 namespace ba {
 __global__ void cam_prep_kernel(Problem, const double *, int);
-__global__ void residual_kernel(Problem, const double *, double *, const double *, double);
-__global__ void jacobian_kernel(Problem, const double *, int);
+template <bool KI> __global__ void residual_kernel(Problem, const double *, double *, const double *, double);
+template <bool KI> __global__ void jacobian_kernel(Problem, const double *, int);
 __global__ void v_kernel(Problem, const double *, const double *);
 __global__ void u_partial_kernel(Problem, const double *, int);
 __global__ void u_final_kernel(Problem, const double *, int);
@@ -195,9 +195,10 @@ struct HostMarks {
 //   mot == 0 : sba_motstr_levmar_x (cameras + points), p = (a_1..a_m, b_1..b_n)
 //   mot == 1 : sba_mot_levmar_x (sba_levmar.c:2090-2690; cameras only), p = (a_1..a_m), the points are read from
 //              `fixed_pts` (n x 3; what sfm_project_point3_mot takes from its adata, sfm.c:553-560) and never change
+// init_params (nullable, m entries): the calibrated-camera fields (known_intrinsics, K_known, k_known) are read.
 static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
                        const double *x, const double *covx, int mnp,
-                       const bsfm_sfm_model_t *model, int jac_mode,
+                       const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, int jac_mode,
                        int itmax, int verbose, const double opts[6], double info[10],
                        int use_constraints, const bsfm_camera_constraints_t *constraints,
                        int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
@@ -427,6 +428,22 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     if (model->f_fixed) BSFM_CUDA_TRY(cudaMemcpyAsync(d_ffixed, model->f_fixed, (size_t) m * sizeof(double), cudaMemcpyHostToDevice, st));
     else BSFM_CUDA_TRY(cudaMemsetAsync(d_ffixed, 0, (size_t) m * sizeof(double), st));
     P.R_init = d_Rinit; P.f_fixed = d_ffixed;
+    // calibrated cameras (sfm.c:339-357): the table exists only when one is present, and selects the KI kernels
+    std::vector<CamIntrinsics> h_intr;
+    if (init_params) {
+        bool any_known = false;
+        for (int j = 0; j < m && !any_known; j++) any_known = init_params[j].known_intrinsics != 0;
+        if (any_known) {
+            h_intr.resize(m);
+            for (int j = 0; j < m; j++) h_intr[j] = cam_intrinsics(init_params[j]);
+            CamIntrinsics *d_intr;
+            TRY(D.alloc(&d_intr, (size_t) m));
+            BSFM_CUDA_TRY(cudaMemcpyAsync(d_intr, h_intr.data(), (size_t) m * sizeof(CamIntrinsics), cudaMemcpyHostToDevice, st));
+            P.intr = d_intr;
+        }
+    }
+    auto *const k_residual = P.intr ? residual_kernel<true> : residual_kernel<false>;
+    auto *const k_jacobian = P.intr ? jacobian_kernel<true> : jacobian_kernel<false>;
     std::vector<char> h_cc; std::vector<double> h_cv, h_cw;
     if (use_constraints) {
         if (!constraints) { set_error("use_constraints set but constraints == NULL"); return BSFM_ERR_ARG; }
@@ -505,7 +522,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     auto launch_residual = [&](const double *pp, double *camR, double *eout, const double *eprev, double eps5v) -> int {
         P.camR = camR;
         BA_LAUNCH(cam_prep_kernel, (m + 127) / 128, 128, P, pp, with_pert);
-        BA_LAUNCH(residual_kernel, red_blocks_obs, 256, P, pp, eout, eprev, eps5v);
+        BA_LAUNCH(k_residual, red_blocks_obs, 256, P, pp, eout, eprev, eps5v);
         return BSFM_OK;
     };
 
@@ -533,7 +550,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     for (itno = 0; itno < itmax && !stop; ++itno) {
         PT.begin(1);
         P.camR = d_camR_a;
-        jacobian_kernel<<<(nvis + 127) / 128, 128, 0, st>>>(P, d_p, jac_mode); ++njev;
+        k_jacobian<<<(nvis + 127) / 128, 128, 0, st>>>(P, d_p, jac_mode); ++njev;
         BSFM_KERNEL_CHECK();
         u_partial_kernel<<<m * useg, 128, 0, st>>>(P, d_e, useg);
         BA_LAUNCH(u_final_kernel, m, 96, P, d_p, useg);
@@ -648,7 +665,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     if (Sout) {
         // export pass (sba_levmar.c:1633-2026): Jacobian at the final p, U/V/W with constraints, UNDAMPED Schur complement
         P.camR = d_camR_a;
-        jacobian_kernel<<<(nvis + 127) / 128, 128, 0, st>>>(P, d_p, jac_mode); ++njev;
+        k_jacobian<<<(nvis + 127) / 128, 128, 0, st>>>(P, d_p, jac_mode); ++njev;
         BSFM_KERNEL_CHECK();
         u_partial_kernel<<<m * useg, 128, 0, st>>>(P, d_e, useg);
         BA_LAUNCH(u_final_kernel, m, 96, P, d_p, useg);
@@ -687,6 +704,19 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     return (stop != 7 && !almost_singular) ? itno : SBA_ERROR_RC;
 }
 
+extern "C" int bsfm_sba_motstr_levmar_model_ki(int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
+                                               const double *x, const double *covx, int mnp,
+                                               const bsfm_sfm_model_t *model, int jac_mode,
+                                               int itmax, int verbose, const double opts[6], double info[10],
+                                               int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                               int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
+                                               double *Vout, double *Sout, double *Uout, double *Wout,
+                                               const bsfm_camera_params_t *init_params)
+{
+    return levmar_impl(0, nullptr, n, m, mcon, vmask, p, cnp, pnp, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
+                       use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout);
+}
+
 extern "C" int bsfm_sba_motstr_levmar_model(int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
                                             const double *x, const double *covx, int mnp,
                                             const bsfm_sfm_model_t *model, int jac_mode,
@@ -695,8 +725,20 @@ extern "C" int bsfm_sba_motstr_levmar_model(int n, int m, int mcon, const char *
                                             int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
                                             double *Vout, double *Sout, double *Uout, double *Wout)
 {
-    return levmar_impl(0, nullptr, n, m, mcon, vmask, p, cnp, pnp, x, covx, mnp, model, jac_mode, itmax, verbose, opts, info,
-                       use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout);
+    return bsfm_sba_motstr_levmar_model_ki(n, m, mcon, vmask, p, cnp, pnp, x, covx, mnp, model, jac_mode, itmax, verbose, opts, info,
+                                           use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout,
+                                           nullptr);
+}
+
+extern "C" int bsfm_sba_mot_levmar_model_ki(int n, int m, int mcon, const char *vmask, double *p, int cnp,
+                                            const double *x, const double *covx, int mnp,
+                                            const bsfm_sfm_model_t *model, const double *points, int jac_mode,
+                                            int itmax, int verbose, const double opts[6], double info[10],
+                                            int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                            const bsfm_camera_params_t *init_params)
+{
+    return levmar_impl(1, points, n, m, mcon, vmask, p, cnp, 3, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
+                       use_constraints, constraints, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
 }
 
 extern "C" int bsfm_sba_mot_levmar_model(int n, int m, int mcon, const char *vmask, double *p, int cnp,
@@ -705,8 +747,8 @@ extern "C" int bsfm_sba_mot_levmar_model(int n, int m, int mcon, const char *vma
                                          int itmax, int verbose, const double opts[6], double info[10],
                                          int use_constraints, const bsfm_camera_constraints_t *constraints)
 {
-    return levmar_impl(1, points, n, m, mcon, vmask, p, cnp, 3, x, covx, mnp, model, jac_mode, itmax, verbose, opts, info,
-                       use_constraints, constraints, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
+    return bsfm_sba_mot_levmar_model_ki(n, m, mcon, vmask, p, cnp, x, covx, mnp, model, points, jac_mode, itmax, verbose, opts, info,
+                                        use_constraints, constraints, nullptr);
 }
 
 // == sba_Axb_Chol, lib/sba-1.5/sba_lapack.c:374-485: x = A^-1 B for symmetric positive definite A (m x m).
@@ -785,8 +827,6 @@ extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask
     if (num_pts <= 0 || num_cameras <= 0 || !vmask || !projections || !init_camera_params || !init_pts) {
         set_error("bsfm_run_sfm: bad arguments"); return BSFM_ERR_ARG;
     }
-    for (int j = 0; j < num_cameras; j++)
-        if (init_camera_params[j].known_intrinsics) { set_error("bsfm_run_sfm: known_intrinsics cameras are outside the GPU path"); return BSFM_ERR_UNSUPPORTED; }
 
     const double f_scale = 0.001, k_scale = 5.0;                 // sfm.c:634-635 (TEST_FOCAL)
     int cnp = est_focal_length ? 7 : 6;
@@ -866,15 +906,15 @@ extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask
     const int verbosity = verb_env ? atoi(verb_env) : 3;          // VERBOSITY 3, MAX_ITERS 150 (sfm.c:814-815)
     int rc;
     if (fix_points)     // sfm.c:843-849: motion-only BA, the points come from init_pts and stay as they are
-        rc = bsfm_sba_mot_levmar_model(num_pts, num_cameras, ncons, vmask, params.data(), cnp, projections, nullptr, 2,
-                                       &model, params.data() + num_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
-                                       use_constraints, use_constraints ? constraints.data() : nullptr);
+        rc = bsfm_sba_mot_levmar_model_ki(num_pts, num_cameras, ncons, vmask, params.data(), cnp, projections, nullptr, 2,
+                                          &model, params.data() + num_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                                          use_constraints, use_constraints ? constraints.data() : nullptr, init_camera_params);
     else
-        rc = bsfm_sba_motstr_levmar_model(num_pts, num_cameras, ncons, vmask, params.data(), cnp, 3, projections, nullptr, 2,
-                                          &model, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
-                                          use_constraints, use_constraints ? constraints.data() : nullptr,
-                                          use_point_constraints, use_point_constraints ? point_constraints.data() : nullptr,
-                                          Vout, Sout, Uout, Wout);
+        rc = bsfm_sba_motstr_levmar_model_ki(num_pts, num_cameras, ncons, vmask, params.data(), cnp, 3, projections, nullptr, 2,
+                                             &model, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                                             use_constraints, use_constraints ? constraints.data() : nullptr,
+                                             use_point_constraints, use_point_constraints ? point_constraints.data() : nullptr,
+                                             Vout, Sout, Uout, Wout, init_camera_params);
     if (rc < -1) {              // BSFM_ERR_*: nothing was solved; the caller's cameras get their scale fields back (they were set
         for (int j = 0; j < num_cameras; j++) { init_camera_params[j].f_scale = 1.0; init_camera_params[j].k_scale = 1.0; }   // to 0.001 / 5 above)
         return rc;

@@ -81,6 +81,75 @@ def ba_scene(num_cameras=50, num_points=20000, views_per_point=5, seed=1234, pix
     return scene
 
 
+def ba_scene_known_intrinsics(num_cameras=20, num_points=2000, views_per_point=5, seed=4321, ordinary_fraction=0.0,
+                              pixel_noise=0.5, pt_noise=0.02, cam_noise=0.01, f_noise=0.01, focal=800.0):
+    """A ba_scene whose cameras are calibrated (camera_params_t::known_intrinsics, lib/sfm-driver/sfm.c:339-357).
+    Every calibrated camera has its own K_known (focal lengths near `focal`, skew, an off-centre principal point) and
+    k_known (radial k0, k1, k4 and tangential k2, k3 all nonzero); its measurements come from that model plus
+    N(0, pixel_noise^2).  A seeded `ordinary_fraction` of the cameras stay focal-only pinhole cameras (measured as in
+    ba_scene).  Adds known [m] int8, K_known [m,9], k_known [m,5] to the ba_scene dict; "f" is the initial focal
+    parameter of every camera (what the radial step and est_focal_length act on).  Use ki_kwargs(scene) to pass the
+    calibration to run_sfm and friends."""
+    rng = np.random.default_rng(seed)
+    m, n, L = num_cameras, num_points, views_per_point
+    ang = 2.0 * np.pi * np.arange(m) / m
+    c = np.stack([6.0 * np.cos(ang), 0.3 * np.sin(3 * ang), 6.0 * np.sin(ang)], 1)
+    R = np.zeros((m, 3, 3))
+    for j in range(m):
+        z = c[j] / np.linalg.norm(c[j])
+        xax = np.cross(np.array([0.0, 1.0, 0.0]), z); xax /= np.linalg.norm(xax)
+        R[j] = np.stack([xax, np.cross(z, xax), z], 0)
+    known = np.ones(m, np.int8)
+    n_ord = int(round(ordinary_fraction * m))
+    if n_ord:
+        known[rng.choice(m, size=n_ord, replace=False)] = 0
+    K_known = np.zeros((m, 3, 3))
+    K_known[:, 0, 0] = focal * (1.0 + 0.05 * rng.standard_normal(m))
+    K_known[:, 0, 1] = rng.uniform(-3.0, 3.0, m)                 # skew
+    K_known[:, 0, 2] = rng.uniform(-25.0, 25.0, m)               # principal point (Bundler's centred pixel frame)
+    K_known[:, 1, 1] = K_known[:, 0, 0] * (1.0 + 0.01 * rng.standard_normal(m))
+    K_known[:, 1, 2] = rng.uniform(-25.0, 25.0, m)
+    K_known[:, 2, 2] = 1.0
+    k_known = np.stack([rng.uniform(-0.12, -0.04, m), rng.uniform(0.01, 0.04, m), rng.uniform(-2e-3, 2e-3, m),
+                        rng.uniform(-2e-3, 2e-3, m), rng.uniform(-4e-3, 4e-3, m)], 1)
+    pts = rng.uniform(-1.0, 1.0, size=(n, 3))
+    vmask = np.zeros((n, m), np.int8)
+    step = max(m // L, 1)
+    starts = (np.arange(n) * 7) % m
+    for k in range(L):
+        vmask[np.arange(n), (starts + k * step) % m] = 1
+    pi, cj = np.nonzero(vmask)
+    Pc = np.einsum("oij,oj->oi", R[cj], pts[pi] - c[cj])
+    proj = -Pc[:, :2] * focal / Pc[:, 2:3]
+    kn = known[cj] != 0
+    x_n, y_n = -Pc[kn, 0] / Pc[kn, 2], -Pc[kn, 1] / Pc[kn, 2]
+    kk, KK = k_known[cj[kn]], K_known[cj[kn]]
+    rsq = x_n * x_n + y_n * y_n
+    factor = 1.0 + kk[:, 0] * rsq + kk[:, 1] * rsq ** 2 + kk[:, 4] * rsq ** 3
+    x_d = x_n * factor + 2 * kk[:, 2] * x_n * y_n + kk[:, 3] * (rsq + 2 * x_n * x_n)
+    y_d = y_n * factor + kk[:, 2] * (rsq + 2 * y_n * y_n) + 2 * kk[:, 3] * x_n * y_n
+    proj[kn, 0] = KK[:, 0, 0] * x_d + KK[:, 0, 1] * y_d + KK[:, 0, 2]
+    proj[kn, 1] = KK[:, 1, 1] * y_d + KK[:, 1, 2]
+    proj = proj + pixel_noise * rng.standard_normal(proj.shape)
+    f0 = np.where(known != 0, K_known[:, 0, 0], focal)
+    return {
+        "vmask": vmask, "projections": np.ascontiguousarray(proj),
+        "gt_pts": pts, "gt_c": c, "gt_R": R.reshape(m, 9).copy(), "gt_f": f0.copy(),
+        "R": R.reshape(m, 9).copy(),
+        "c": c + cam_noise * rng.standard_normal(c.shape),
+        "f": f0 * (1.0 + f_noise * rng.standard_normal(m)),
+        "k": np.zeros((m, 2)),
+        "pts": pts + pt_noise * rng.standard_normal(pts.shape),
+        "known": known, "K_known": K_known.reshape(m, 9).copy(), "k_known": k_known,
+    }
+
+
+def ki_kwargs(scene):
+    """the calibration keywords (known, K_known, k_known) of a scene for run_sfm / call_run_sfm / reprojection_rmse /
+    reprojection_outliers; empty for a scene without calibrated cameras"""
+    return {k: scene[k] for k in ("known", "K_known", "k_known") if k in scene}
+
+
 def write_key_file(path, desc, seed=0):
     """Lowe text .key file (src/keys2a.cpp:183-253): "<num> 128", then per key "<y> <x> <scale> <ori>" and the
     128 descriptor values in 7 lines of 20,20,20,20,20,20,8 integers."""

@@ -102,13 +102,37 @@ int bsfm_sba_mot_levmar_model(int n, int m, int mcon, const char *vmask, double 
                               int itmax, int verbose, const double opts[6], double info[10],
                               int use_constraints, const bsfm_camera_constraints_t *constraints);
 
+/* The two solvers above with calibrated cameras.  init_params (nullable, m entries) is what sfm_project_point3 reads
+ * from its adata besides the model: a camera with known_intrinsics != 0 projects through its own K_known[0,1,2,4,5]
+ * and Brown-Conrady k_known[0..4] instead of the focal-only pinhole (lib/sfm-driver/sfm.c:339-357), followed by the
+ * same optional radial step, which still uses the focal parameter (aj[6] / f_scale or f_fixed[j]) and aj's k1, k2.
+ * Only known_intrinsics, K_known and k_known are read; cameras may be mixed.  Unlike vmask, p and x, init_params is
+ * read on the host during setup and must be host memory.  With init_params == NULL, or with no
+ * calibrated camera in it, these are exactly bsfm_sba_motstr_levmar_model / bsfm_sba_mot_levmar_model, which call
+ * them with NULL.  Both Jacobian modes cover calibrated cameras.                                                 */
+int bsfm_sba_motstr_levmar_model_ki(int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
+                                    const double *x, const double *covx, int mnp,
+                                    const bsfm_sfm_model_t *model, int jac_mode,
+                                    int itmax, int verbose, const double opts[6], double info[10],
+                                    int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                    int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
+                                    double *Vout, double *Sout, double *Uout, double *Wout,
+                                    const bsfm_camera_params_t *init_params);
+int bsfm_sba_mot_levmar_model_ki(int n, int m, int mcon, const char *vmask, double *p, int cnp,
+                                 const double *x, const double *covx, int mnp,
+                                 const bsfm_sfm_model_t *model, const double *points, int jac_mode,
+                                 int itmax, int verbose, const double opts[6], double info[10],
+                                 int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                 const bsfm_camera_params_t *init_params);
+
 /* == run_sfm (lib/sfm-driver/sfm.h:68-86): same arguments, same in/out semantics
  * (init_camera_params and init_pts are overwritten with the solution, sfm.c:876-929; prints
  * "[run_sfm] Number of iterations" / "info[6]" like sfm.c:872-873), plus `info_out` (nullable,
  * 10 doubles) and an int return (0 or negative error) which the void reference lacks.
- * fix_points == 1 runs the motion-only solver (sfm.c:843-849; init_pts untouched).  GPU path covers
- * optimize_for_fisheye == 0, const_focal_length == 0 and cameras with known_intrinsics == 0; anything else
- * returns BSFM_ERR_UNSUPPORTED.                                                                 */
+ * fix_points == 1 runs the motion-only solver (sfm.c:843-849; init_pts untouched).  Cameras with
+ * known_intrinsics != 0 project through their K_known / k_known (see bsfm_sba_motstr_levmar_model_ki), which
+ * run_sfm neither packs nor changes.  GPU path covers optimize_for_fisheye == 0 and const_focal_length == 0;
+ * anything else returns BSFM_ERR_UNSUPPORTED.                                                   */
 int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask, double *projections,
                  int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
                  bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
@@ -124,7 +148,8 @@ int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask, double *p
  *   outliers    : every point with dist > thresh in some camera, unless pt_protected[point] != 0 (the caller's
  *                 "constrained point" rule, :801-806); the reported error is the distance in the first (lowest
  *                 index) camera that flags the point, like the reference's first-found rule (:809-821)
- * cameras: the `R`, `t` (= centre), `f`, `k` fields of run_sfm's output are read.
+ * cameras: the `R`, `t` (= centre), `f`, `k` fields of run_sfm's output are read, and for cameras with known_intrinsics
+ *   != 0 also K_known and k_known (sfm.c:339-357, then the radial step with f and k).  fisheye cameras are refused.
  * cam_stats (nullable): num_cameras x 5 = { #observations, mean distance, median (iround(0.5 n)-th), med80, thresh }
  * obs_dist  (nullable): one distance per observation in the order of `projections`
  * outliers / outlier_errors: up to `cap` entries, ordered by (first flagging camera, point index) -- the

@@ -44,7 +44,6 @@ static int model_from_globals(const char *fn, const bsfm_sfm_global_t *g, int m,
     *f_fixed = (double *) malloc((size_t) m * sizeof(double));
     if (!*R_init || !*f_fixed) { fprintf(stderr, "SBA/b200: %s(): out of memory\n", fn); exit(1); }
     for (j = 0; j < m; j++) {
-        if (g->init_params[j].known_intrinsics) { free(*R_init); free(*f_fixed); return unsupported(fn, "known_intrinsics cameras are outside the GPU path"); }
         if (g->init_params[j].f_scale != g->init_params[0].f_scale || g->init_params[j].k_scale != g->init_params[0].k_scale) {
             free(*R_init); free(*f_fixed); return unsupported(fn, "per-camera f_scale / k_scale differ");
         }
@@ -91,8 +90,10 @@ int sba_motstr_levmar_x(const int n, const int m, const int mcon, char *vmask, d
     rc = model_from_globals(fn, (const bsfm_sfm_global_t *) wd->adata, m, cnp, &model, &R_init, &f_fixed);
     if (rc) return rc;
     /* opts really has 6 entries for the Bundler build of sba (it reads opts[5], sba_levmar.c:610) */
-    rc = bsfm_sba_motstr_levmar_model(n, m, mcon, vmask, p, cnp, pnp, x, NULL, mnp, &model, BSFM_BA_JAC_FD, itmax, verbose, opts, info,
-                                      use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout);
+    /* calibrated cameras: sfm_project_point3 reads known_intrinsics / K_known / k_known from the same init_params */
+    rc = bsfm_sba_motstr_levmar_model_ki(n, m, mcon, vmask, p, cnp, pnp, x, NULL, mnp, &model, BSFM_BA_JAC_FD, itmax, verbose, opts, info,
+                                         use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout,
+                                         ((const bsfm_sfm_global_t *) wd->adata)->init_params);
     free(R_init); free(f_fixed);
     return finish(fn, rc);
 }
@@ -150,8 +151,8 @@ int sba_mot_levmar_x(const int n, const int m, const int mcon, char *vmask, doub
     rc = model_from_globals(fn, g, m, cnp, &model, &R_init, &f_fixed);
     if (rc) return rc;
     if (!g->points) { free(R_init); free(f_fixed); return unsupported(fn, "adata->points is NULL"); }
-    rc = bsfm_sba_mot_levmar_model(n, m, mcon, vmask, p, cnp, x, NULL, mnp, &model, (const double *) g->points, BSFM_BA_JAC_FD, itmax, verbose, opts, info,
-                                   use_constraints, constraints);
+    rc = bsfm_sba_mot_levmar_model_ki(n, m, mcon, vmask, p, cnp, x, NULL, mnp, &model, (const double *) g->points, BSFM_BA_JAC_FD, itmax, verbose,
+                                      opts, info, use_constraints, constraints, g->init_params);
     free(R_init); free(f_fixed);
     return finish(fn, rc);
 }

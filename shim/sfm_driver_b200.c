@@ -8,8 +8,7 @@
  *     ... -o bundler ... sfm_driver_b200.o -L<repo>/bundler_sfm_b200 -lbsfm_b200   (instead of -lsfmdrv -lsba.v1.5)
  *
  * The struct arguments are layout-identical (include/bsfm_b200_ba.h restates camera_params_t / v3_t).
- * Options the GPU path does not cover (fisheye, known_intrinsics) terminate like the reference's own fatal
- * paths do (printf + exit(1), sfm.c:56-73): there is deliberately no silent CPU fallback.
+ * Options the GPU path does not cover (fisheye) terminate like the reference's own fatal paths do (printf + exit(1), sfm.c:56-73): there is deliberately no silent CPU fallback.
  */
 #include <math.h>
 #include <stdio.h>
@@ -59,7 +58,6 @@ void sfm_project_point3(int j, int i, double *aj, double *bi, double *xij, void 
     const double *dt = aj, *w = aj + 3, *k = aj + (g->est_focal_length ? 7 : 6);
     double f, R[9], b2[3], bc[3];
     (void) i;
-    if (init->known_intrinsics) { printf("[sfm_project_point3/b200] known_intrinsics cameras are not supported\n"); exit(1); }
     if (!g->est_focal_length) f = init->f;
     else if (g->const_focal_length) { printf("Error: case of constant focal length has not been implemented.\n"); f = g->global_params.f; }
     else f = aj[6] / init->f_scale;
@@ -74,9 +72,23 @@ void sfm_project_point3(int j, int i, double *aj, double *bi, double *xij, void 
         bc[1] = R[3] * b2[0] + R[4] * b2[1] + R[5] * b2[2];
         bc[2] = R[6] * b2[0] + R[7] * b2[1] + R[8] * b2[2];
     }
-    xij[0] = -bc[0] * f / bc[2];
-    xij[1] = -bc[1] * f / bc[2];
-    if (g->estimate_distortion) {
+    if (!init->known_intrinsics) {
+        xij[0] = -bc[0] * f / bc[2];
+        xij[1] = -bc[1] * f / bc[2];
+    } else {    /* calibrated camera: Brown-Conrady k_known, then K_known (sfm.c:339-357) */
+        const double *kk = init->k_known, *K = init->K_known;
+        const double x_n = -bc[0] / bc[2];
+        const double y_n = -bc[1] / bc[2];
+        const double rsq = x_n * x_n + y_n * y_n;
+        const double factor = 1.0 + kk[0] * rsq + kk[1] * rsq * rsq + kk[4] * rsq * rsq * rsq;
+        const double dx_x = 2 * kk[2] * x_n * y_n + kk[3] * (rsq + 2 * x_n * x_n);
+        const double dx_y = kk[2] * (rsq + 2 * y_n * y_n) + 2 * kk[3] * x_n * y_n;
+        const double x_d = x_n * factor + dx_x;
+        const double y_d = y_n * factor + dx_y;
+        xij[0] = K[0] * x_d + K[1] * y_d + K[2];
+        xij[1] = K[4] * y_d + K[5];
+    }
+    if (g->estimate_distortion) {     /* the radial step runs for both kinds of camera and uses f (sfm.c:362-377) */
         const double k1 = k[0] / init->k_scale, k2 = k[1] / init->k_scale;
         const double rsq = (xij[0] * xij[0] + xij[1] * xij[1]) / (f * f);
         const double factor = 1.0 + k1 * rsq + k2 * rsq * rsq;
