@@ -192,6 +192,51 @@ def test_mid_size_system_uses_blocked_path_vs_oracle(oracle):
     check_solution(got, ref, scene["projections"].shape[0], "mid200")
 
 
+@pytest.mark.parametrize("ncons", [0, 2])
+def test_tile_kernel_system_vs_reference(ncons, monkeypatch):
+    """150 cameras -> reduced system 1350 x 1350 (1332 with two fixed cameras): the fused-step Cholesky whose first steps run
+    chol_tile_kernel, the regime every Bundler reconstruction passes through between ~139 and ~170 free cameras.
+
+    Both sides stop through Snavely's stop-8 rule (max_i |e_i - e'_i| / |e_i| < eps5 = 0.04 after >= 4 iterations,
+    sba_levmar.c:1569-1572).  Near convergence that statistic is the largest of 45k residual ratios and hovers just above
+    0.04: on this scene the reference logs 0.0439 at iteration 29, 0.0476 at 31 and 0.0194 at 34 (stop after 34; with two
+    fixed cameras 0.0431 at 31 and 0.0348 at 33), and a reference linked against a different BLAS stopped the same solve at 36.
+    Which iteration stops is decided by rounding.  So the trajectory is compared at an equal iteration count with stop-8
+    disabled on both sides (as test_config3_equal_iteration_count_vs_reference does): iterations, linear systems, error and
+    parameters must agree.  The full solves are compared on error, stop reason and an iteration count within 3; their
+    parameters are not, because after a different number of iterations they differ along the weakly determined directions
+    (the similarity gauge when no camera is fixed)."""
+    from oracle import loader
+    from tests import ba_restatement as rs
+    from tests.test_ba_normal_equations import gpu_motstr
+    if loader.ref_sba() is None:
+        pytest.skip("needs oracle/_ref (REF_SBA_ITMAX / REF_SBA_EPS5 of the unmodified reference)")
+    scene = synth.ba_scene(150, 4500, 5, seed=17)
+    nvis = scene["projections"].shape[0]
+    # equal iteration count: 30 iterations (past where stop-8 first comes close), eps5 = 0 on both sides
+    monkeypatch.setenv("REF_SBA_ITMAX", "30")
+    monkeypatch.setenv("REF_SBA_EPS5", "0")
+    ref = loader.run_sfm_ref(scene, ncons=ncons)
+    P = rs.problem(scene, ncons=ncons)
+    rc, p, info, _ = gpu_motstr(P, P.p0, 0, 30, eps5=0.0)
+    assert rc == 30 and int(info[5]) == int(ref["info"][5]) == 30 and int(info[6]) == int(ref["info"][6]) == 3
+    assert int(info[9]) == int(ref["info"][9])                             # same number of linear systems solved
+    assert abs(info[0] - ref["info"][0]) <= 1e-9 * abs(ref["info"][0])
+    assert abs(np.sqrt(info[1] / nvis) - np.sqrt(ref["info"][1] / nvis)) <= RMSE_TOL
+    sol = rs.unpack(P, p)
+    for key in ("R", "c", "f", "pts"):
+        assert rel_group_err(sol[key], ref[key]) <= PARAM_TOL, (key, rel_group_err(sol[key], ref[key]))
+    assert np.array_equal(sol["c"][:ncons], scene["c"][:ncons])
+    # the full solves
+    monkeypatch.delenv("REF_SBA_ITMAX")
+    monkeypatch.delenv("REF_SBA_EPS5")
+    got = bundle.run_sfm(scene, ncons=ncons)
+    ref = loader.run_sfm_ref(scene, ncons=ncons)
+    assert abs(np.sqrt(got["info"][1] / nvis) - np.sqrt(ref["info"][1] / nvis)) <= RMSE_TOL
+    assert int(got["info"][6]) == int(ref["info"][6]) == 8
+    assert abs(int(got["info"][5]) - int(ref["info"][5])) <= 3, (got["info"][5], ref["info"][5])
+
+
 def test_odd_pitch_system_vs_oracle(oracle):
     """cnp = 7 with 221 cameras -> reduced system dimension 1547 (> 1536: large path; odd row pitch: scalar access path)"""
     scene = synth.ba_scene(221, 4000, 5, seed=8)
@@ -221,11 +266,16 @@ def _axb_chol(A, b):
     return fn(A.ctypes.data, b.ctypes.data, x.ctypes.data, A.shape[0], 0), x
 
 
-@pytest.mark.parametrize("n", [9, 33, 64, 65, 255, 321, 450, 640, 641, 1547, 2100, 4000])
+# The fused-step path (641..1536) has three regimes (ba_chol.cu: chol_solve): every step one chol_step_kernel launch that fits
+# in one wave (<= 1024: 1 + 527 CTAs at step 0 against 4 resident 512-thread CTAs per SM on 132 SMs), the same launches with more
+# CTAs than one wave (1025..1248), and steps with more than 800 tiles split into chol_step_kernel<<<1>>> + chol_tile_kernel
+# (1249..1536: the first 1 to 9 steps).
+@pytest.mark.parametrize("n", [9, 33, 64, 65, 255, 321, 450, 640, 641, 1024, 1100, 1248, 1249, 1350, 1503, 1536, 1547, 2100, 4000])
 def test_axb_chol_vs_lapack(n):
     """single tile (<= 32), the one-launch dataflow path (<= 640, incl. partial last tiles and the two-tiles-per-CTA regime), the
-    fused-step path (<= 1536) and the 256-column panel path with the fp64 tensor-core trailing update (> 1536), incl. an odd
-    dimension and one that is not a multiple of 32: backward error at the level of LAPACK's, solution close to LAPACK's"""
+    fused-step path (<= 1536: single wave, multi-wave, and the tile-kernel steps, incl. a last block of 1 row at 1249 and nine
+    tile-kernel steps at 1536) and the 256-column panel path with the fp64 tensor-core trailing update (> 1536), incl. odd
+    dimensions and ones that are not a multiple of 32: backward error at the level of LAPACK's, solution close to LAPACK's"""
     A = _spd(n, seed=n)
     xt = np.random.default_rng(1).standard_normal(n)
     b = A @ xt
@@ -251,12 +301,24 @@ def test_axb_chol_vs_reference_routine():
     assert np.linalg.norm(x - xr) / np.linalg.norm(xr) <= 1e-7
 
 
-@pytest.mark.parametrize("n", [300, 2000])
+@pytest.mark.parametrize("n", [300, 1100, 1350, 2000])
 def test_axb_chol_reports_indefinite_matrix(n):
-    """the reference returns 0 when a leading minor is not positive definite (sba_lapack.c:439-442)"""
+    """the reference returns 0 when a leading minor is not positive definite (sba_lapack.c:439-442), with the bad pivot in the
+    middle: the dataflow path, a multi-wave fused step (1100), a fused step after four tile-kernel steps (1350) and the panel
+    path (the tile-kernel steps themselves: test_axb_chol_reports_bad_pivot_in_tile_kernel_regime)"""
     A = _spd(n, seed=5)
     A[n // 2, n // 2] = -1.0
     rc, _ = _axb_chol(A, np.ones(n))
+    assert rc == 0
+
+
+@pytest.mark.parametrize("where", [5, 200, 1530])
+def test_axb_chol_reports_bad_pivot_in_tile_kernel_regime(where):
+    """n = 1536 (steps 0..8 split into a diagonal-only chol_step launch + chol_tile_kernel): a non-positive pivot in step 0's
+    diagonal-only launch, inside a tile-kernel step, and in the final fused launch"""
+    A = _spd(1536, seed=7)
+    A[where, where] = -1.0
+    rc, _ = _axb_chol(A, np.ones(1536))
     assert rc == 0
 
 

@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 from bundler_sfm_b200 import bundle, synth
+from tests.ba_restatement import port_run_sfm     # numpy restatement of run_sfm, with the calibrated branch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ba_known_intrinsics_golden.npz")
@@ -118,237 +119,6 @@ def check_solution(got, ref, nvis, what, fixed_pts=None, known=None, est_focal=1
     assert abs(got["info"][0] - ref["info"][0]) <= 1e-9 * abs(ref["info"][0]), (what, "initial error")
     if fixed_pts is not None:
         assert np.array_equal(got["pts"], fixed_pts), (what, "points must stay fixed")
-
-
-# ---- CPU restatement of run_sfm -> sba_motstr_levmar_x for calibrated cameras ---------------------------------------------
-# The same restatement as oracle/ba_oracle.c (run_sfm, sfm.c:592-1003; sba_motstr_levmar_x, sba_levmar.c:457-2081; forward
-# differences, sba_levmar_wrap.c:163-259), in numpy, with the known_intrinsics branch of sfm_project_rd (sfm.c:339-357).
-# Dense Schur complement and LAPACK Cholesky (the reference's dpotrf); sums run in a different order than the reference's,
-# so results agree to rounding.  Motion + structure only (fix_points = 0), like ba_oracle.c.
-def _rot_update_rows(R0, w):       # sfm.c:77-116 for every row of w (N x 3), R0 (N x 9)
-    th = np.sqrt(w[:, 0] * w[:, 0] + w[:, 1] * w[:, 1] + w[:, 2] * w[:, 2])
-    out = R0.reshape(-1, 3, 3).copy()
-    nz = th != 0.0
-    if nz.any():
-        n = w[nz] / th[nz, None]
-        z = np.zeros(n.shape[0])
-        nx = np.stack([z, -n[:, 2], n[:, 1], n[:, 2], z, -n[:, 0], -n[:, 1], n[:, 0], z], 1).reshape(-1, 3, 3)
-        dR = np.eye(3)[None] + nx * np.sin(th[nz])[:, None, None] + (nx @ nx) * (1.0 - np.cos(th[nz]))[:, None, None]
-        out[nz] = dR @ out[nz]
-    return out.reshape(-1, 9)
-
-
-def _project_rows(a, b, R, f_fixed, kn, Kk, kk, est_focal, undistort, explicit_centers, f_scale=0.001, k_scale=5.0):
-    """sfm_project_point3 for N observations: a (N x cnp), b (N x 3), R = rot_update(R_init, w) (N x 9)"""
-    R = R.reshape(-1, 3, 3)
-    if explicit_centers:
-        bc = np.einsum("nij,nj->ni", R, b - a[:, 0:3])
-    else:
-        bc = np.einsum("nij,nj->ni", R, b) + a[:, 0:3]
-    K0 = a[:, 6] / f_scale if est_focal else f_fixed
-    p = np.empty((a.shape[0], 2))
-    p[:, 0] = -bc[:, 0] * K0 / bc[:, 2]
-    p[:, 1] = -bc[:, 1] * K0 / bc[:, 2]
-    if kn.any():
-        p[kn] = bundle.project_known(bc[kn], Kk[kn], kk[kn])
-    if undistort:
-        c = 7 if est_focal else 6
-        k1, k2 = a[:, c] / k_scale, a[:, c + 1] / k_scale
-        rsq = (p[:, 0] * p[:, 0] + p[:, 1] * p[:, 1]) / (K0 * K0)
-        p *= (1.0 + k1 * rsq + k2 * rsq * rsq)[:, None]
-    return p
-
-
-def _fd_step(v):                   # sba_levmar_wrap.c:207-212
-    return np.maximum(np.abs(1e-4 * v), 1e-6)
-
-
-def port_run_sfm(scene, est_focal_length=1, undistort=1, explicit_camera_centers=1, ncons=0, eps2=1e-12,
-                 use_constraints=0, constrained=None, constraints=None, weights=None, use_point_constraints=0,
-                 points_constraints=None, point_constraint_weight=0.0, known=None, K_known=None, k_known=None):
-    f_scale, k_scale = 0.001, 5.0
-    vm = np.asarray(scene["vmask"]) != 0
-    n, m = vm.shape
-    cnp = 6 + (1 if est_focal_length else 0) + (2 if undistort else 0)
-    ncp = m * cnp
-    mcon = ncons
-    pi, cj = np.nonzero(vm)                          # point-major, ascending camera (sba_levmar.c:652-663)
-    nvis = len(pi)
-    x = np.asarray(scene["projections"], float)
-    R_init = np.asarray(scene["R"], float).reshape(m, 9)
-    f_fixed = np.asarray(scene["f"], float)
-    kn = np.zeros(m, bool) if known is None else np.asarray(known) != 0
-    Kk = np.zeros((m, 9)) if K_known is None else np.asarray(K_known, float).reshape(m, 9)
-    kk = np.zeros((m, 5)) if k_known is None else np.asarray(k_known, float).reshape(m, 5)
-    a0 = np.zeros((m, cnp))                          # packing, sfm.c:652-703
-    a0[:, 0:3] = scene["c"]
-    if est_focal_length:
-        a0[:, 6] = f_fixed * f_scale
-    if undistort:
-        c = 7 if est_focal_length else 6
-        a0[:, c:c + 2] = np.asarray(scene["k"], float) * k_scale
-    p = np.concatenate([a0.reshape(-1), np.asarray(scene["pts"], float).reshape(-1)])
-    nvars = p.shape[0]
-    cc = np.zeros((m, cnp), bool); cv = np.zeros((m, cnp)); cw = np.zeros((m, cnp))
-    if use_constraints:                              # sfm.c:721-754
-        cc = np.asarray(constrained)[:, :cnp] != 0
-        cv = np.asarray(constraints, float)[:, :cnp].copy(); cw = np.asarray(weights, float)[:, :cnp].copy()
-        if est_focal_length:
-            cv[:, 6] *= f_scale; cw[:, 6] *= 1.0 / (f_scale * f_scale)
-        if undistort:
-            c = 7 if est_focal_length else 6
-            cv[:, c:c + 2] *= k_scale; cw[:, c:c + 2] *= 1.0 / (k_scale * k_scale)
-    pc = np.zeros(n, bool); pv = np.zeros((n, 3))
-    if use_point_constraints:                        # sfm.c:757-781
-        pv = np.asarray(points_constraints, float)
-        pc = ~np.all(pv == 0.0, axis=1)
-    pw = point_constraint_weight
-
-    def penalty(pp):                                 # sba_levmar.c:808-842
-        acc = 0.0
-        if use_constraints:
-            d = cv - pp[:ncp].reshape(m, cnp)
-            acc += float(np.sum(np.where(cc, cw * d * d, 0.0)))
-        if use_point_constraints:
-            d = pv - pp[ncp:].reshape(n, 3)
-            acc += float(np.sum(nvis * pw * d[pc] * d[pc]))
-        return acc
-
-    def evaluate(pp, a=None, b=None, R=None):
-        A_ = pp[:ncp].reshape(m, cnp)[cj] if a is None else a
-        B_ = pp[ncp:].reshape(n, 3)[pi] if b is None else b
-        R_ = _rot_update_rows(R_init[cj], A_[:, 3:6]) if R is None else R
-        return _project_rows(A_, B_, R_, f_fixed[cj], kn[cj], Kk[cj], kk[cj], est_focal_length, undistort, explicit_camera_centers)
-
-    opts = (1.0e-3, 1.0e-10, eps2, 1.0e-12, 0.0, 4.0e-2)           # sfm.c:705-714
-    tau, eps1, eps2_, eps3_sq, eps4_sq, eps5 = abs(opts[0]), abs(opts[1]), abs(opts[2]), opts[3] ** 2, opts[4] ** 2, opts[5]
-    eps2_sq = opts[2] * opts[2]
-    e = x - evaluate(p)
-    p_eL2 = float(np.sum(e * e)) + penalty(p)
-    init_p_eL2 = p_eL2
-    nfev, njev, nlss, stop, nu, mu, dp_L2, maxdiag, eab_inf = 1, 0, 0, 0, 2, 0.0, np.finfo(float).max, np.finfo(float).tiny, 0.0
-    if not np.isfinite(p_eL2):
-        stop = 7
-    itno = 0
-    sel = cj >= mcon
-    while itno < 150 and not stop:
-        a = p[:ncp].reshape(m, cnp)[cj]; b = p[ncp:].reshape(n, 3)[pi]
-        R = _rot_update_rows(R_init[cj], a[:, 3:6])
-        h0 = evaluate(p, a, b, R)
-        A = np.zeros((nvis, 2, cnp)); B = np.zeros((nvis, 2, 3))
-        for jj in range(cnp):                        # sba_levmar_wrap.c:203-256
-            d = _fd_step(a[:, jj]); a2 = a.copy(); a2[:, jj] = a[:, jj] + d
-            R2 = _rot_update_rows(R_init[cj], a2[:, 3:6]) if 3 <= jj <= 5 else R
-            A[:, :, jj] = (evaluate(p, a2, b, R2) - h0) * (1.0 / d)[:, None]
-        for jj in range(3):
-            d = _fd_step(b[:, jj]); b2 = b.copy(); b2[:, jj] = b[:, jj] + d
-            B[:, :, jj] = (evaluate(p, a, b2, R) - h0) * (1.0 / d)[:, None]
-        njev += 1
-        U = np.zeros((m, cnp, cnp)); ea = np.zeros((m, cnp))
-        np.add.at(U, cj[sel], np.einsum("oki,okj->oij", A[sel], A[sel]))
-        np.add.at(ea, cj[sel], np.einsum("oki,ok->oi", A[sel], e[sel]))
-        for j in range(mcon, m):                     # sba_levmar.c:952-963
-            d = cv[j] - p[j * cnp:(j + 1) * cnp]
-            U[j][np.diag_indices(cnp)] += np.where(cc[j], cw[j], 0.0)
-            ea[j] += np.where(cc[j], cw[j] * d, 0.0)
-        V = np.zeros((n, 3, 3)); eb = np.zeros((n, 3))
-        np.add.at(V, pi, np.einsum("oki,okj->oij", B, B))
-        np.add.at(eb, pi, np.einsum("oki,ok->oi", B, e))
-        d = pv - p[ncp:].reshape(n, 3)
-        V[pc] += (nvis * pw) * np.eye(3)[None]
-        eb[pc] += nvis * pw * d[pc]
-        W = np.einsum("oki,okj->oij", A, B)
-        W[~sel] = 0.0
-        eab = np.concatenate([ea.reshape(-1), eb.reshape(-1)])
-        eab_inf = float(np.max(np.abs(eab))); p_L2 = float(np.sum(p * p))
-        maxdiag = max(np.finfo(float).tiny, float(np.max(np.diagonal(U[mcon:], axis1=1, axis2=2), initial=0.0)),
-                      float(np.max(np.diagonal(V, axis1=1, axis2=2))))
-        if eab_inf <= eps1:
-            dp_L2 = 0.0; stop = 1; break
-        if itno == 0:
-            mu = tau * maxdiag
-        while True:                                  # damping loop, sba_levmar.c:1131-1597
-            accepted = False
-            Vd = V + mu * np.eye(3)[None]
-            det = np.linalg.det(Vd)
-            if not np.all(np.isfinite(det) & (det != 0.0)):
-                pass                                 # singular V*_i: more damping (:1156-1161)
-            else:
-                Vinv = np.linalg.inv(Vd)
-                Y = W @ Vinv[pi]                      # Y_ij = W_ij V*_i^-1
-                Sd = (m - mcon) * cnp
-                S = np.zeros((m, cnp, m, cnp))
-                for j in range(mcon, m):
-                    S[j, :, j, :] = U[j] + mu * np.eye(cnp)
-                E = ea.copy()
-                np.add.at(E, cj[sel], -np.einsum("oij,oj->oi", Y[sel], eb[pi[sel]]))
-                for i in range(n):                   # S_jk -= sum_i Y_ij W_ik^T
-                    os_ = np.nonzero((pi == i) & sel)[0]
-                    if len(os_):
-                        blk = np.einsum("aik,bjk->aibj", Y[os_], W[os_])
-                        S[np.ix_(cj[os_], range(cnp), cj[os_], range(cnp))] -= blk
-                Sm = S[mcon:, :, mcon:, :].reshape(Sd, Sd)
-                nlss += 1
-                try:
-                    L = np.linalg.cholesky(Sm)
-                    da = np.linalg.solve(L.T, np.linalg.solve(L, E[mcon:].reshape(-1)))
-                    solved = True
-                except np.linalg.LinAlgError:
-                    solved = False
-                if solved:
-                    dp = np.zeros(nvars)
-                    dp[mcon * cnp:ncp] = da
-                    dacam = dp[:ncp].reshape(m, cnp)
-                    wt = np.zeros((n, 3))
-                    np.add.at(wt, pi[sel], np.einsum("oji,oj->oi", W[sel], dacam[cj[sel]]))
-                    dp[ncp:] = np.einsum("nij,nj->ni", Vinv, eb - wt).reshape(-1)
-                    pdp = p + dp
-                    dp_L2 = float(np.sum(dp * dp))
-                    if dp_L2 <= eps2_sq * p_L2:
-                        stop = 2; break
-                    if dp_L2 >= (p_L2 + eps2_) / (1e-12 * 1e-12):
-                        return None                  # almost singular: the reference returns SBA_ERROR
-                    hx = x - evaluate(pdp); nfev += 1
-                    pdp_eL2 = float(np.sum(hx * hx))
-                    if not np.isfinite(pdp_eL2):
-                        stop = 7; break
-                    pdp_eL2 += penalty(p)            # constraint terms at the OLD p (:1487-1522)
-                    dL = float(np.sum(dp * (mu * dp + eab)))
-                    dF = p_eL2 - pdp_eL2
-                    if dL > 0.0 and dF > 0.0:
-                        tmp = 2.0 * dF / dL - 1.0
-                        tmp = 1.0 - tmp * tmp * tmp
-                        mu = mu * (tmp if tmp >= 0.3333333334 else 0.3333333334)
-                        nu = 2
-                        ef, hf = e.reshape(-1), hx.reshape(-1)
-                        chk = ~((ef < eps5) & (hf < eps5))
-                        with np.errstate(divide="ignore", invalid="ignore"):
-                            pct = np.abs((ef[chk] - hf[chk]) / ef[chk])
-                        max_pct = float(np.max(pct, initial=0.0))
-                        if pdp_eL2 - 2.0 * np.sqrt(p_eL2 * pdp_eL2) < (eps4_sq - 1.0) * p_eL2:
-                            stop = 4
-                        if max_pct < eps5 and itno >= 4:
-                            stop = 8; break
-                        p, e, p_eL2 = pdp, hx, pdp_eL2
-                        accepted = True
-            if accepted:
-                break
-            mu *= nu                                 # :1584-1597 (int nu overflows after 2^30)
-            if nu >= 1 << 30:
-                stop = 6; break
-            nu <<= 1
-        if p_eL2 <= eps3_sq:
-            stop = 5
-        itno += 1
-    if itno >= 150:
-        stop = 3
-    info = np.array([init_p_eL2, p_eL2, eab_inf, dp_L2, mu / maxdiag, itno, stop, nfev, njev, nlss], float)
-    a = p[:ncp].reshape(m, cnp)                      # unpacking, sfm.c:876-929
-    Rout = _rot_update_rows(R_init, a[:, 3:6])
-    f = a[:, 6] / f_scale if est_focal_length else f_fixed.copy()
-    c = 7 if est_focal_length else 6
-    k = a[:, c:c + 2] / k_scale if undistort else np.asarray(scene["k"], float).copy()
-    return {"R": Rout, "c": a[:, 0:3].copy(), "f": f, "k": k, "pts": p[ncp:].reshape(n, 3).copy(), "info": info}
 
 
 # ---- CPU: the golden file against the numpy restatement -------------------------------------------------------------
@@ -493,7 +263,7 @@ def _ref_or_skip():
     from oracle import loader
     if loader.ref_sba() is None:
         pytest.skip("oracle/_ref/libref_sba.so not available (oracle.run_sfm_oracle's C restatement has no calibrated-camera "
-                    "branch; port_run_sfm above is pinned to the golden file instead)")
+                    "branch; port_run_sfm of tests/ba_restatement.py is pinned to the golden file instead)")
     return loader
 
 
