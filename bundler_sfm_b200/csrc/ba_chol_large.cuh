@@ -21,6 +21,10 @@ inline size_t chol_extra_ws_doubles(int n)
     // small systems: (n + 1) x n behind the scratch; large ones finish their last panels with the dataflow kernel: room for its largest case
     return (size_t) ((n + LNBO - 1) / LNBO) * LNBO * LNBO + (size_t) n + 64 + (size_t) (std::min(n, DF_MAX_N) + 1) * std::min(n, DF_MAX_N) + 64;
 }
+// doubles of the whole linv_ws workspace chol_solve takes for an n x n system: the 32 x 32 inverses, then the above
+inline size_t chol_ws_doubles(int n) { return (size_t) ((n + LNB - 1) / LNB) * LNB * LNB + chol_extra_ws_doubles(n); }
+// symmetric A (both triangles) + right-hand side in row n, factor out of place in Lmat, solution in x (ba_chol.cu)
+int chol_solve(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *x, Scalars *sc);
 // where the large path keeps that scratch inside linv_ws
 inline size_t chol_large_pub_offset(int n) { return (size_t) ((n + LNB - 1) / LNB) * LNB * LNB + (size_t) ((n + LNBO - 1) / LNBO) * LNBO * LNBO + (size_t) n + 64; }
 int chol_dataflow_factor(cudaStream_t st, const double *A, double *Lmat, int ld, int n, double *linv_blocks, double *pub, Scalars *sc, bool *used);

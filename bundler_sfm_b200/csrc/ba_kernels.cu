@@ -937,82 +937,6 @@ __global__ void update_kernel(Problem P, const double *p, double *pdp)
     if (grid_reduce<0>(dl, P.partial + gridDim.x, P.ticket + 1, out)) P.sc->dL = out;
 }
 
-// ------------------------------------------------------------------------------------------------
-// structure-building kernels (setup): vmask -> CRS, Schur tuples
-// ------------------------------------------------------------------------------------------------
-__global__ void vmask_count_kernel(const char *vmask, int n, int m, int *row_count)
-{
-    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (i >= n) return;
-    int c = 0;
-    for (int j = lane; j < m; j += 32) c += vmask[(size_t) i * m + j] != 0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
-    if (lane == 0) row_count[i] = c;
-}
-
-__global__ void vmask_fill_kernel(const char *vmask, int n, int m, const int *rowptr, int *obs_cam, int *obs_pt)
-{
-    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (i >= n) return;
-    int pos = rowptr[i];
-    for (int j0 = 0; j0 < m; j0 += 32) {
-        const int j = j0 + lane;
-        const bool v = j < m && vmask[(size_t) i * m + j] != 0;
-        const unsigned ball = __ballot_sync(0xffffffffu, v);
-        if (v) {
-            const int q = pos + __popc(ball & ((1u << lane) - 1u));
-            obs_cam[q] = j; obs_pt[q] = i;
-        }
-        pos += __popc(ball);
-    }
-}
-
-// tuples of point i: all (a <= b) pairs of its observations restricted to cameras >= mcon
-__global__ void tuple_count_kernel(int n, int mcon, const int *rowptr, const int *obs_cam, int *tuple_count)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int L = 0;
-    for (int o = rowptr[i]; o < rowptr[i + 1]; o++) L += obs_cam[o] >= mcon;
-    tuple_count[i] = L * (L + 1) / 2;
-}
-
-__global__ void tuple_fill_kernel(int n, int m, int mcon, const int *rowptr, const int *obs_cam, const int *tuple_off,
-                                  uint32_t *keys, int2 *vals)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int pos = tuple_off[i];
-    const int r0 = rowptr[i], r1 = rowptr[i + 1];
-    for (int a = r0; a < r1; a++) {
-        const int ja = obs_cam[a];
-        if (ja < mcon) continue;
-        for (int b = a; b < r1; b++) {
-            const int jb = obs_cam[b];   // ascending camera order inside a row => ja <= jb
-            keys[pos] = (uint32_t) ja * (uint32_t) m + (uint32_t) jb;
-            vals[pos] = make_int2(a, b);
-            pos++;
-        }
-    }
-}
-
-// sorted (obs_a, obs_b) -> (obs_a, obs_b, point, 0)
-__global__ void tuple_expand_kernel(const int2 *in, const int *obs_pt, int4 *out, int count)
-{
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q < count) { const int2 v = in[q]; out[q] = make_int4(v.x, v.y, obs_pt[v.x], 0); }
-}
-
-__global__ void chunk_count_kernel(const int *blk_cnt, int nblocks, int *chunk_cnt)
-{
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < nblocks) chunk_cnt[b] = (blk_cnt[b] + SCHUR_CHUNK - 1) / SCHUR_CHUNK;
-    else if (b == nblocks) chunk_cnt[b] = 0;
-}
-
 // Wout export (sba_levmar.c:1835-1846): dense (m*cnp) x (3n) matrix, W_ij at rows j*cnp.., columns 3i..
 __global__ void wout_scatter_kernel(Problem P, double *Wout)
 {
@@ -1043,12 +967,6 @@ __global__ void vinv_export_kernel(Problem P)
     O[0] = c00 * id; O[1] = c01 * id; O[2] = c02 * id;
     O[3] = c01 * id; O[4] = (a00 * a22 - a02 * a02) * id; O[5] = (a01 * a02 - a00 * a12) * id;
     O[6] = c02 * id; O[7] = O[5]; O[8] = (a00 * a11 - a01 * a01) * id;
-}
-
-__global__ void iota_kernel(int *v, int count)
-{
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q < count) v[q] = q;
 }
 
 }  // namespace ba

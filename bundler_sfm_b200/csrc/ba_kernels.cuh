@@ -143,5 +143,24 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, c
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
+// kernels of ba_kernels.cu that the LM solver (ba_solver.cu) launches
+__global__ void cam_prep_kernel(Problem P, const double *p, int with_pert);
+template <bool KI> __global__ void residual_kernel(Problem P, const double *p, double *e_out, const double *e_prev, double eps5);
+template <bool KI> __global__ void jacobian_kernel(Problem P, const double *p, int jac_mode);
+__global__ void v_kernel(Problem P, const double *p, const double *e);
+__global__ void u_partial_kernel(Problem P, const double *e, int nseg);
+__global__ void u_final_kernel(Problem P, const double *p, int nseg);
+__global__ void grad_stats_kernel(Problem P, const double *p);
+__global__ void penalty_kernel(Problem P, const double *p);
+__global__ void vinv_kernel(Problem P);
+__global__ void schur_partial_kernel(Problem P);
+__global__ void schur_final_kernel(Problem P);
+__global__ void zero_kernel(double *ptr, size_t count);
+__global__ void backsub_kernel(Problem P, const double *da);
+__global__ void update_kernel(Problem P, const double *p, double *pdp);
+__global__ void mot_solve_kernel(Problem P);
+__global__ void wout_scatter_kernel(Problem P, double *Wout);
+__global__ void vinv_export_kernel(Problem P);
+
 }  // namespace ba
 }  // namespace bsfm

@@ -13,17 +13,15 @@
 #include <cstring>
 #include <vector>
 
-#include <cub/cub.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 
 #include "common.h"
 #include "ba_kernels.cuh"
+#include "ba_setup.h"
 #include "../../include/bsfm_b200_ba.h"
 
 namespace bsfm {
 namespace ba {
-
-__global__ void vmask_count_kernel(const char *, int, int, int *);
-__global__ void vmask_fill_kernel(const char *, int, int, const int *, int *, int *);
 
 struct CamCompact { double R[9], t[3], f, k0, k1; };
 
@@ -59,24 +57,10 @@ __global__ void outlier_dist_kernel(int nvis, const int *obs_cam, const int *obs
     dist[o] = sqrt(dx * dx + dy * dy);     // Bundle.cpp:753-756
 }
 
-__global__ void outlier_iota_kernel(int *v, int count)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < count) v[i] = i;
-}
 __global__ void outlier_gather_kernel(int count, const int *idx, const double *src, double *dst)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count) dst[i] = src[idx[i]];
-}
-// cam_ptr[j] = first position of camera j in the camera-sorted key array
-__global__ void outlier_cam_ptr_kernel(const int *sorted_cam, int nvis, int m, int *cam_ptr)
-{
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j > m) return;
-    int lo = 0, hi = nvis;     // first index with sorted_cam[idx] >= j
-    while (lo < hi) { const int mid = (lo + hi) >> 1; if (sorted_cam[mid] < j) lo = mid + 1; else hi = mid; }
-    cam_ptr[j] = lo;
 }
 
 __device__ __forceinline__ int iround_dev(double x) { return (x < 0.0) ? (int) (x - 0.5) : (int) (x + 0.5); }   // util.c:75-81
@@ -120,20 +104,6 @@ __global__ void outlier_err_kernel(int nvis, const int *obs_cam, const int *obs_
     if (first_cam[i] == obs_cam[o]) err[i] = dist[o];
 }
 
-namespace {
-struct DevBuf {
-    std::vector<void *> ptrs;
-    ~DevBuf() { for (void *p : ptrs) cudaFree(p); }
-    template <typename T> cudaError_t alloc(T **out, size_t count)
-    {
-        void *p = nullptr;
-        cudaError_t e = cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T));
-        if (e == cudaSuccess) { ptrs.push_back(p); *out = (T *) p; }
-        return e;
-    }
-};
-}  // namespace
-
 }  // namespace ba
 }  // namespace bsfm
 
@@ -159,35 +129,13 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
         any_known = any_known || cams[j].known_intrinsics;
     }
 
-    DevBuf D;
-    char *d_vmask, *d_prot = nullptr;
-    int *d_rowcnt, *d_rowptr, *d_obs_cam, *d_obs_pt;
-    BSFM_CUDA_TRY(D.alloc(&d_vmask, (size_t) n * m));
-    BSFM_CUDA_TRY(D.alloc(&d_rowcnt, (size_t) n + 1));
-    BSFM_CUDA_TRY(D.alloc(&d_rowptr, (size_t) n + 1));
-    BSFM_CUDA_TRY(cudaMemcpy(d_vmask, vmask, (size_t) n * m, cudaMemcpyDefault));
-    BSFM_CUDA_TRY(cudaMemset(d_rowcnt, 0, ((size_t) n + 1) * sizeof(int)));
-    vmask_count_kernel<<<(n * 32 + 255) / 256, 256>>>(d_vmask, n, m, d_rowcnt);
-    BSFM_KERNEL_CHECK();
-    void *d_tmp = nullptr; size_t tmp_bytes = 0;
-    auto ensure_tmp = [&](size_t need) -> cudaError_t {
-        if (need <= tmp_bytes) return cudaSuccess;
-        char *q; cudaError_t e = D.alloc(&q, need); if (e == cudaSuccess) { d_tmp = q; tmp_bytes = need; } return e;
-    };
-    {
-        size_t need = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, need, d_rowcnt, d_rowptr, n + 1);
-        BSFM_CUDA_TRY(ensure_tmp(need));
-        BSFM_CUDA_TRY(cub::DeviceScan::ExclusiveSum(d_tmp, need, d_rowcnt, d_rowptr, n + 1));
-        count_launch(2);
-    }
-    int nvis = 0;
-    BSFM_CUDA_TRY(cudaMemcpy(&nvis, d_rowptr + n, sizeof(int), cudaMemcpyDeviceToHost));
+    // the legacy default stream, as every copy below: callers may pass device pointers written on it
+    DeviceArena D(0);
+    Visibility vis;
+    TRY(build_visibility(vmask, n, m, 0, D, vis));
+    const int nvis = vis.nvis;
     if (nvis <= 0) { set_error("bsfm_reprojection_outliers: empty visibility mask"); return BSFM_ERR_ARG; }
-    BSFM_CUDA_TRY(D.alloc(&d_obs_cam, (size_t) nvis));
-    BSFM_CUDA_TRY(D.alloc(&d_obs_pt, (size_t) nvis));
-    vmask_fill_kernel<<<(n * 32 + 255) / 256, 256>>>(d_vmask, n, m, d_rowptr, d_obs_cam, d_obs_pt);
-    BSFM_KERNEL_CHECK();
+    int *d_obs_cam = vis.obs_cam, *d_obs_pt = vis.obs_pt, *d_cam_obs = vis.cam_obs, *d_cam_ptr = vis.cam_ptr;
 
     // cameras (what the loop reads: R, t = centre, f, k), points, measurements
     std::vector<CamCompact> hc(m);
@@ -196,55 +144,30 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
         hc[j].f = cams[j].f; hc[j].k0 = cams[j].k[0]; hc[j].k1 = cams[j].k[1];
     }
     CamCompact *d_cams; double *d_pts, *d_proj, *d_dist, *d_dist_cam, *d_dist_sorted, *d_stats, *d_err;
-    int *d_iota, *d_cam_obs, *d_cam_sorted, *d_cam_ptr, *d_first;
-    BSFM_CUDA_TRY(D.alloc(&d_cams, (size_t) m));
-    BSFM_CUDA_TRY(D.alloc(&d_pts, (size_t) n * 3));
-    BSFM_CUDA_TRY(D.alloc(&d_proj, (size_t) nvis * 2));
-    BSFM_CUDA_TRY(D.alloc(&d_dist, (size_t) nvis)); BSFM_CUDA_TRY(D.alloc(&d_dist_cam, (size_t) nvis)); BSFM_CUDA_TRY(D.alloc(&d_dist_sorted, (size_t) nvis));
-    BSFM_CUDA_TRY(D.alloc(&d_stats, (size_t) m * 5)); BSFM_CUDA_TRY(D.alloc(&d_err, (size_t) n));
-    BSFM_CUDA_TRY(D.alloc(&d_iota, (size_t) nvis)); BSFM_CUDA_TRY(D.alloc(&d_cam_obs, (size_t) nvis)); BSFM_CUDA_TRY(D.alloc(&d_cam_sorted, (size_t) nvis));
-    BSFM_CUDA_TRY(D.alloc(&d_cam_ptr, (size_t) m + 1)); BSFM_CUDA_TRY(D.alloc(&d_first, (size_t) n));
-    BSFM_CUDA_TRY(cudaMemcpy(d_cams, hc.data(), (size_t) m * sizeof(CamCompact), cudaMemcpyHostToDevice));
+    char *d_prot = nullptr;
+    int *d_first;
+    TRY(D.alloc(&d_dist, (size_t) nvis)); TRY(D.alloc(&d_dist_cam, (size_t) nvis)); TRY(D.alloc(&d_dist_sorted, (size_t) nvis));
+    TRY(D.alloc(&d_stats, (size_t) m * 5)); TRY(D.alloc(&d_err, (size_t) n));
+    TRY(D.alloc(&d_first, (size_t) n));
+    TRY(D.upload(&d_cams, hc.data(), (size_t) m));
     CamIntrinsics *d_intr = nullptr;     // calibrated cameras (sfm.c:339-357): side table, only when there is one
     if (any_known) {
         std::vector<CamIntrinsics> hi(m);
         for (int j = 0; j < m; j++) hi[j] = cam_intrinsics(cams[j]);
-        BSFM_CUDA_TRY(D.alloc(&d_intr, (size_t) m));
-        BSFM_CUDA_TRY(cudaMemcpy(d_intr, hi.data(), (size_t) m * sizeof(CamIntrinsics), cudaMemcpyHostToDevice));
+        TRY(D.upload(&d_intr, hi.data(), (size_t) m));
     }
-    BSFM_CUDA_TRY(cudaMemcpy(d_pts, pts, (size_t) n * 3 * sizeof(double), cudaMemcpyDefault));
-    BSFM_CUDA_TRY(cudaMemcpy(d_proj, projections, (size_t) nvis * 2 * sizeof(double), cudaMemcpyDefault));
-    if (pt_protected) {
-        BSFM_CUDA_TRY(D.alloc(&d_prot, (size_t) n));
-        BSFM_CUDA_TRY(cudaMemcpy(d_prot, pt_protected, (size_t) n, cudaMemcpyDefault));
-    }
+    TRY(D.upload(&d_pts, pts, (size_t) n * 3));
+    TRY(D.upload(&d_proj, projections, (size_t) nvis * 2));
+    if (pt_protected) TRY(D.upload(&d_prot, pt_protected, (size_t) n));
     const int gb = (nvis + 255) / 256;
     if (d_intr) outlier_dist_kernel<true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
     else outlier_dist_kernel<false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
     BSFM_KERNEL_CHECK();
 
-    // camera-major view (stable sort by camera keeps ascending point order), per-camera sorted distances
-    outlier_iota_kernel<<<gb, 256>>>(d_iota, nvis);
-    BSFM_KERNEL_CHECK();
-    {
-        int bits = 1; while ((1LL << bits) < m) bits++;
-        size_t need = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, need, d_obs_cam, d_cam_sorted, d_iota, d_cam_obs, nvis, 0, bits);
-        BSFM_CUDA_TRY(ensure_tmp(need));
-        BSFM_CUDA_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, need, d_obs_cam, d_cam_sorted, d_iota, d_cam_obs, nvis, 0, bits));
-        count_launch(3);
-    }
-    outlier_cam_ptr_kernel<<<(m + 1 + 255) / 256, 256>>>(d_cam_sorted, nvis, m, d_cam_ptr);
-    BSFM_KERNEL_CHECK();
+    // per-camera sorted distances, in the camera-major view (ascending point order within each camera)
     outlier_gather_kernel<<<gb, 256>>>(nvis, d_cam_obs, d_dist, d_dist_cam);
     BSFM_KERNEL_CHECK();
-    {
-        size_t need = 0;
-        cub::DeviceSegmentedSort::SortKeys(nullptr, need, d_dist_cam, d_dist_sorted, nvis, m, d_cam_ptr, d_cam_ptr + 1);
-        BSFM_CUDA_TRY(ensure_tmp(need));
-        BSFM_CUDA_TRY(cub::DeviceSegmentedSort::SortKeys(d_tmp, need, d_dist_cam, d_dist_sorted, nvis, m, d_cam_ptr, d_cam_ptr + 1));
-        count_launch(3);
-    }
+    TRY(D.cub(3, [&](void *t, size_t &b) { return cub::DeviceSegmentedSort::SortKeys(t, b, d_dist_cam, d_dist_sorted, nvis, m, d_cam_ptr, d_cam_ptr + 1); }));
     outlier_cam_stats_kernel<<<(m * 32 + 255) / 256, 256>>>(m, d_cam_ptr, d_dist_cam, d_dist_sorted, min_proj_error_threshold, max_proj_error_threshold, d_stats);
     BSFM_KERNEL_CHECK();
     BSFM_CUDA_TRY(cudaMemset(d_first, 0x7f, (size_t) n * sizeof(int)));      // 0x7f7f7f7f: larger than any camera index

@@ -1,0 +1,281 @@
+// ba_setup.cu -- setup of a BA call (ba_setup.h): device memory pool, visibility mask -> CRS and camera-major permutation,
+// Schur structure, and the kernels that build them.
+#include "ba_setup.h"
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_run_length_encode.cuh>
+#include <cub/device/device_scan.cuh>
+#include <cstdlib>
+#include <map>
+#include <mutex>
+
+namespace bsfm {
+namespace ba {
+
+// structure-building kernels: vmask -> CRS, camera-major permutation, Schur tuples
+__global__ void vmask_count_kernel(const char *vmask, int n, int m, int *row_count)
+{
+    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;
+    int c = 0;
+    for (int j = lane; j < m; j += 32) c += vmask[(size_t) i * m + j] != 0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
+    if (lane == 0) row_count[i] = c;
+}
+
+__global__ void vmask_fill_kernel(const char *vmask, int n, int m, const int *rowptr, int *obs_cam, int *obs_pt)
+{
+    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;
+    int pos = rowptr[i];
+    for (int j0 = 0; j0 < m; j0 += 32) {
+        const int j = j0 + lane;
+        const bool v = j < m && vmask[(size_t) i * m + j] != 0;
+        const unsigned ball = __ballot_sync(0xffffffffu, v);
+        if (v) {
+            const int q = pos + __popc(ball & ((1u << lane) - 1u));
+            obs_cam[q] = j; obs_pt[q] = i;
+        }
+        pos += __popc(ball);
+    }
+}
+
+// obs_pt from the CRS row pointers (the host-scanned visibility mask below): one warp per point
+__global__ void csr_rows_kernel(const int *rowptr, int n, int *obs_pt)
+{
+    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;
+    for (int q = rowptr[i] + lane; q < rowptr[i + 1]; q += 32) obs_pt[q] = i;
+}
+
+__global__ void iota_kernel(int *v, int count)
+{
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < count) v[q] = q;
+}
+
+// cam_ptr[j] = first position of camera j in the camera-sorted key array
+__global__ void cam_ptr_kernel(const int *sorted_cam, int nvis, int m, int *cam_ptr)
+{
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j > m) return;
+    int lo = 0, hi = nvis;   // first position with cam >= j
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (sorted_cam[mid] < j) lo = mid + 1; else hi = mid;
+    }
+    cam_ptr[j] = lo;
+}
+
+// tuples of point i: all (a <= b) pairs of its observations restricted to cameras >= mcon
+__global__ void tuple_count_kernel(int n, int mcon, const int *rowptr, const int *obs_cam, int *tuple_count)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    int L = 0;
+    for (int o = rowptr[i]; o < rowptr[i + 1]; o++) L += obs_cam[o] >= mcon;
+    tuple_count[i] = L * (L + 1) / 2;
+}
+
+__global__ void tuple_fill_kernel(int n, int m, int mcon, const int *rowptr, const int *obs_cam, const int *tuple_off,
+                                  uint32_t *keys, int2 *vals)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    int pos = tuple_off[i];
+    const int r0 = rowptr[i], r1 = rowptr[i + 1];
+    for (int a = r0; a < r1; a++) {
+        const int ja = obs_cam[a];
+        if (ja < mcon) continue;
+        for (int b = a; b < r1; b++) {
+            const int jb = obs_cam[b];   // ascending camera order inside a row => ja <= jb
+            keys[pos] = (uint32_t) ja * (uint32_t) m + (uint32_t) jb;
+            vals[pos] = make_int2(a, b);
+            pos++;
+        }
+    }
+}
+
+// sorted (obs_a, obs_b) -> (obs_a, obs_b, point, 0)
+__global__ void tuple_expand_kernel(const int2 *in, const int *obs_pt, int4 *out, int count)
+{
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < count) { const int2 v = in[q]; out[q] = make_int4(v.x, v.y, obs_pt[v.x], 0); }
+}
+
+__global__ void chunk_count_kernel(const int *blk_cnt, int nblocks, int *chunk_cnt)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < nblocks) chunk_cnt[b] = (blk_cnt[b] + SCHUR_CHUNK - 1) / SCHUR_CHUNK;
+    else if (b == nblocks) chunk_cnt[b] = 0;
+}
+
+namespace {
+// Device blocks are recycled across calls (RunSFM_SBA calls run_sfm once per outlier round on a problem of
+// nearly the same size, src/Bundle.cpp:586-913): cudaMalloc/cudaFree cost tens of microseconds each and a solve of the
+// 50-camera configuration only takes milliseconds.  Blocks return to a per-process pool when a call ends.
+struct BlockPool {
+    std::mutex mu;
+    std::multimap<size_t, void *> free_blocks;   // capacity -> pointer
+    size_t pooled_bytes = 0;
+    int device = -1;
+    void bind_device(int dev)   // blocks belong to one device: drop the pool when the caller switches GPUs
+    {
+        std::lock_guard<std::mutex> g(mu);
+        if (dev == device) return;
+        for (auto &kv : free_blocks) cudaFree(kv.second);
+        free_blocks.clear(); pooled_bytes = 0; device = dev;
+    }
+    void *get(size_t bytes, size_t *cap_out)
+    {
+        std::lock_guard<std::mutex> g(mu);
+        auto it = free_blocks.lower_bound(bytes);
+        if (it != free_blocks.end() && it->first <= bytes + bytes / 4 + 4096) {
+            void *p = it->second; *cap_out = it->first; pooled_bytes -= it->first;
+            free_blocks.erase(it);
+            return p;
+        }
+        return nullptr;
+    }
+    void put(void *p, size_t cap)
+    {
+        std::lock_guard<std::mutex> g(mu);
+        if (pooled_bytes + cap > ((size_t) 24 << 30)) { cudaFree(p); return; }   // bound what the pool may hold
+        free_blocks.emplace(cap, p); pooled_bytes += cap;
+    }
+};
+BlockPool g_pool;
+}  // namespace
+
+DeviceArena::~DeviceArena()
+{
+    if (!blocks.empty()) cudaStreamSynchronize(st);
+    for (auto &b : blocks) g_pool.put(b.first, b.second);
+}
+
+int DeviceArena::alloc_bytes(void **out, size_t bytes)
+{
+    if (blocks.empty()) { int dev = 0; BSFM_CUDA_TRY(cudaGetDevice(&dev)); g_pool.bind_device(dev); }
+    bytes = (bytes + 255) & ~(size_t) 255;
+    size_t cap = bytes;
+    void *p = g_pool.get(bytes, &cap);
+    if (!p) {
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes): %s", bytes, cudaGetErrorString(e)); return BSFM_ERR_CUDA; }
+        cap = bytes;
+    }
+    blocks.push_back({p, cap});
+    *out = p;
+    return BSFM_OK;
+}
+
+// visibility: vmask -> CRS (sba_levmar.c:652-663), camera-major permutation
+int build_visibility(const char *vmask, int n, int m, cudaStream_t st, DeviceArena &D, Visibility &V)
+{
+    // host-resident masks of at least BSFM_BA_MASK_HOST_MIN bytes are scanned on the host and only their CRS form is uploaded
+    // (host_scan_vmask, common.cpp).  OFF by default: at config 3 it cuts the H2D bytes per solve from 560 to 75 MB, but the scan
+    // of the 500 MB mask costs host time, and whether it beats the PCIe copy from pinned memory depends on the host.
+    static const size_t host_scan_min = []() { const char *e = getenv("BSFM_BA_MASK_HOST_MIN"); return e ? (size_t) atoll(e) : ~(size_t) 0; }();
+    bool host_mask = false;
+    if ((size_t) n * m >= host_scan_min) {
+        cudaPointerAttributes pa;
+        if (cudaPointerGetAttributes(&pa, vmask) == cudaSuccess) host_mask = (pa.type == cudaMemoryTypeHost || pa.type == cudaMemoryTypeUnregistered);
+        else cudaGetLastError();
+    }
+    char *d_vmask = nullptr;
+    int *d_rowcnt;
+    std::vector<int> h_rowptr, h_obs_cam;
+    TRY(D.alloc(&d_rowcnt, (size_t) n + 1));
+    TRY(D.alloc(&V.rowptr, (size_t) n + 1));
+    if (host_mask) {
+        host_scan_vmask(vmask, n, m, h_rowptr, h_obs_cam);
+        BSFM_CUDA_TRY(cudaMemcpyAsync(V.rowptr, h_rowptr.data(), ((size_t) n + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+        V.nvis = h_rowptr[n];
+    } else {
+        TRY(D.upload(&d_vmask, vmask, (size_t) n * m));   // host or device pointer (UVA)
+        BSFM_CUDA_TRY(cudaMemsetAsync(d_rowcnt, 0, ((size_t) n + 1) * sizeof(int), st));
+        vmask_count_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(d_vmask, n, m, d_rowcnt);
+        BSFM_KERNEL_CHECK();
+        TRY(D.cub(2, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, d_rowcnt, V.rowptr, n + 1, st); }));
+        BSFM_CUDA_TRY(cudaMemcpyAsync(&V.nvis, V.rowptr + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+        BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    const int nvis = V.nvis;
+    if (nvis <= 0) return BSFM_OK;
+    int *d_iota, *d_cam_sorted;
+    TRY(D.alloc(&V.obs_cam, (size_t) nvis)); TRY(D.alloc(&V.obs_pt, (size_t) nvis));
+    TRY(D.alloc(&V.cam_ptr, (size_t) m + 1)); TRY(D.alloc(&V.cam_obs, (size_t) nvis)); TRY(D.alloc(&d_iota, (size_t) nvis));
+    if (host_mask) {
+        BSFM_CUDA_TRY(cudaMemcpyAsync(V.obs_cam, h_obs_cam.data(), (size_t) nvis * sizeof(int), cudaMemcpyHostToDevice, st));
+        csr_rows_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(V.rowptr, n, V.obs_pt);
+    } else {
+        vmask_fill_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(d_vmask, n, m, V.rowptr, V.obs_cam, V.obs_pt);
+    }
+    BSFM_KERNEL_CHECK();
+    // camera-major permutation: stable sort of observation ids by camera.  The int keys sort as they are: cub's signed-key
+    // transform flips bit 31 only, outside the sorted bits [0, bits).
+    TRY(D.alloc(&d_cam_sorted, (size_t) nvis));
+    iota_kernel<<<(nvis + 255) / 256, 256, 0, st>>>(d_iota, nvis);
+    BSFM_KERNEL_CHECK();
+    int bits = 1; while ((1LL << bits) < m) bits++;
+    TRY(D.cub(3, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, V.obs_cam, d_cam_sorted, d_iota, V.cam_obs, nvis, 0, bits, st); }));
+    cam_ptr_kernel<<<(m + 1 + 255) / 256, 256, 0, st>>>(d_cam_sorted, nvis, m, V.cam_ptr);
+    BSFM_KERNEL_CHECK();
+    return BSFM_OK;
+}
+
+// Schur structure: (obs_a, obs_b) tuples of every point, sorted by block key j*m+k (stable => ascending point)
+int build_schur_structure(Problem &P, cudaStream_t st, DeviceArena &D)
+{
+    const int n = P.n, m = P.m, mcon = P.mcon;
+    int *d_tcnt, *d_toff;
+    TRY(D.alloc(&d_tcnt, (size_t) n + 1)); TRY(D.alloc(&d_toff, (size_t) n + 1));
+    BSFM_CUDA_TRY(cudaMemsetAsync(d_tcnt, 0, ((size_t) n + 1) * sizeof(int), st));
+    tuple_count_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, mcon, P.rowptr, P.obs_cam, d_tcnt);
+    BSFM_KERNEL_CHECK();
+    TRY(D.cub(2, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, d_tcnt, d_toff, n + 1, st); }));
+    int ntuples = 0;
+    BSFM_CUDA_TRY(cudaMemcpyAsync(&ntuples, d_toff + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+    BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+    uint32_t *d_tkey_a, *d_tkey_b, *d_blk_key;
+    unsigned long long *d_tval_a, *d_tval_b;
+    int *d_blk_cnt, *d_blk_start, *d_nruns;
+    TRY(D.alloc(&d_tkey_a, (size_t) ntuples)); TRY(D.alloc(&d_tkey_b, (size_t) ntuples));
+    TRY(D.alloc(&d_tval_a, (size_t) ntuples)); TRY(D.alloc(&d_tval_b, (size_t) ntuples));
+    const int max_blocks = (int) std::min<int64_t>((int64_t) ntuples, (int64_t) (m - mcon) * (m - mcon + 1) / 2);
+    TRY(D.alloc(&d_blk_key, (size_t) max_blocks + 1)); TRY(D.alloc(&d_blk_cnt, (size_t) max_blocks + 1));
+    TRY(D.alloc(&d_blk_start, (size_t) max_blocks + 2)); TRY(D.alloc(&d_nruns, 1));
+    tuple_fill_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, m, mcon, P.rowptr, P.obs_cam, d_toff, d_tkey_a, (int2 *) d_tval_a);
+    BSFM_KERNEL_CHECK();
+    int bits = 1; while ((1LL << bits) < (long long) m * m) bits++;
+    TRY(D.cub(3, [&](void *t, size_t &b) { return cub::DeviceRadixSort::SortPairs(t, b, d_tkey_a, d_tkey_b, d_tval_a, d_tval_b, ntuples, 0, bits, st); }));
+    TRY(D.cub(2, [&](void *t, size_t &b) { return cub::DeviceRunLengthEncode::Encode(t, b, d_tkey_b, d_blk_key, d_blk_cnt, d_nruns, ntuples, st); }));
+    int nblocks = 0;
+    BSFM_CUDA_TRY(cudaMemcpyAsync(&nblocks, d_nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
+    BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+    BSFM_CUDA_TRY(cudaMemsetAsync(d_blk_cnt + nblocks, 0, sizeof(int), st));
+    TRY(D.cub(2, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, d_blk_cnt, d_blk_start, nblocks + 1, st); }));
+    // chunk list (SCHUR_CHUNK tuples per partial-sum warp) + (obs_a, obs_b, point) tuples
+    int *d_chunk_cnt, *d_chunk_off;
+    int4 *d_tuples4;
+    TRY(D.alloc(&d_chunk_cnt, (size_t) nblocks + 1)); TRY(D.alloc(&d_chunk_off, (size_t) nblocks + 1));
+    TRY(D.alloc(&d_tuples4, (size_t) ntuples));
+    chunk_count_kernel<<<(nblocks + 1 + 255) / 256, 256, 0, st>>>(d_blk_cnt, nblocks, d_chunk_cnt);
+    BSFM_KERNEL_CHECK();
+    TRY(D.cub(2, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, d_chunk_cnt, d_chunk_off, nblocks + 1, st); }));
+    tuple_expand_kernel<<<(ntuples + 255) / 256, 256, 0, st>>>((const int2 *) d_tval_b, P.obs_pt, d_tuples4, ntuples);
+    BSFM_KERNEL_CHECK();
+    int nchunks = 0;
+    BSFM_CUDA_TRY(cudaMemcpyAsync(&nchunks, d_chunk_off + nblocks, sizeof(int), cudaMemcpyDeviceToHost, st));
+    BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+    P.nblocks = nblocks; P.blk_key = d_blk_key; P.blk_start = d_blk_start; P.tuples = d_tuples4;
+    P.nchunks = nchunks; P.chunk_off = d_chunk_off;
+    TRY(D.alloc(&P.schur_part, (size_t) nchunks * SCHUR_PART_STRIDE));
+    return BSFM_OK;
+}
+
+}  // namespace ba
+}  // namespace bsfm

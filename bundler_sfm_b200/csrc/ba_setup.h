@@ -1,0 +1,73 @@
+// ba_setup.h -- host side of the BA setup, shared by the LM solver (ba_solver.cu) and the outlier pass (ba_outliers.cu):
+// pooled device memory, cub's two-phase calls, and the structures built once per call from the visibility mask.
+#pragma once
+#include <algorithm>
+#include <utility>
+#include <vector>
+#include "common.h"
+#include "ba_kernels.cuh"
+
+#define TRY(expr) do { int rc__ = (expr); if (rc__ != BSFM_OK) return rc__; } while (0)
+
+namespace bsfm {
+namespace ba {
+
+// Device memory of one call, recycled through a process-wide pool of the current device's blocks.  The pool serves every
+// thread, so the destructor waits for `st`, the stream that uses the blocks, before returning them: an error return with
+// work in flight must not hand them to another call while that work still writes them.
+struct DeviceArena {
+    explicit DeviceArena(cudaStream_t s) : st(s) {}
+    ~DeviceArena();
+    DeviceArena(const DeviceArena &) = delete;
+    DeviceArena &operator=(const DeviceArena &) = delete;
+    template <typename T> int alloc(T **out, size_t count)
+    {
+        void *p;
+        TRY(alloc_bytes(&p, std::max<size_t>(count, 1) * sizeof(T)));
+        *out = (T *) p;
+        return BSFM_OK;
+    }
+    // alloc + copy of `count` elements from host or device memory, on st
+    template <typename T> int upload(T **out, const void *src, size_t count)
+    {
+        TRY(alloc(out, count));
+        BSFM_CUDA_TRY(cudaMemcpyAsync((void *) *out, src, count * sizeof(T), cudaMemcpyDefault, st));
+        return BSFM_OK;
+    }
+    // cub's two-phase call: call(temp, bytes) sizes its scratch (grown here, kept for later calls), then does the work
+    // in `launches` kernels
+    template <typename F> int cub(int launches, F call)
+    {
+        size_t need = 0;
+        BSFM_CUDA_TRY(call(nullptr, need));
+        if (need > scratch_bytes) { char *q; TRY(alloc(&q, need)); scratch = q; scratch_bytes = need; }
+        BSFM_CUDA_TRY(call(scratch, need));
+        count_launch(launches);
+        return BSFM_OK;
+    }
+    const cudaStream_t st;
+
+private:
+    int alloc_bytes(void **out, size_t bytes);
+    std::vector<std::pair<void *, size_t>> blocks;
+    void *scratch = nullptr;
+    size_t scratch_bytes = 0;
+};
+
+// Which cameras see which points (idxij, sba_levmar.c:652-663); the arrays exist only when nvis > 0
+struct Visibility {
+    int nvis = 0;
+    int *rowptr = nullptr;    // n + 1, point-major CRS
+    int *obs_cam = nullptr;   // nvis, ascending camera within each point
+    int *obs_pt = nullptr;    // nvis
+    int *cam_obs = nullptr;   // nvis, observation ids grouped by camera, ascending point within each camera
+    int *cam_ptr = nullptr;   // m + 1: camera j's observations are cam_obs[cam_ptr[j] .. cam_ptr[j + 1])
+};
+// from the dense n x m mask of the reference interface, a host or device pointer; synchronises `st` once to learn nvis
+int build_visibility(const char *vmask, int n, int m, cudaStream_t st, DeviceArena &D, Visibility &V);
+
+// Schur structure of P's visibility: fills P.nblocks, blk_key, blk_start, tuples, nchunks, chunk_off and schur_part
+int build_schur_structure(Problem &P, cudaStream_t st, DeviceArena &D);
+
+}  // namespace ba
+}  // namespace bsfm

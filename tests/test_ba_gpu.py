@@ -366,22 +366,26 @@ def test_axb_chol_large_path_lookahead_equals_serial_order():
 
 
 def test_host_compressed_visibility_mask_equals_uploaded_mask():
-    """large host-resident masks are scanned on the host and uploaded as CRS (ba_solver.cu: host_scan_vmask); forced here on a
-    small scene (BSFM_BA_MASK_HOST_MIN=1, 3 scan threads) and compared bit for bit with the dense upload, in child processes"""
+    """large host-resident masks are scanned on the host and uploaded as CRS (ba_setup.cu: build_visibility, host_scan_vmask);
+    forced here on a small scene (BSFM_BA_MASK_HOST_MIN=1, 3 scan threads) and compared bit for bit with the dense upload, for
+    the solve and for the outlier pass on the solved scene, in child processes"""
     import subprocess
     import sys
     import tempfile
     code = ("import numpy as np, sys; sys.path.insert(0, %r); from bundler_sfm_b200 import bundle, synth; "
             "sc = synth.ba_scene(12, 3000, 5, seed=3); out = bundle.run_sfm(sc); "
-            "np.savez(sys.argv[1], info=out['info'], R=out['R'], c=out['c'], f=out['f'], k=out['k'], pts=out['pts'])") % ROOT
+            "ol = bundle.reprojection_outliers(dict(sc, R=out['R'], c=out['c'], f=out['f'], k=out['k'], pts=out['pts']), 1, 2.0, 16.0); "
+            "np.savez(sys.argv[1], info=out['info'], R=out['R'], c=out['c'], f=out['f'], k=out['k'], pts=out['pts'], "
+            "dist=ol['dist'], stats=ol['stats'], outliers=ol['outliers'], errors=ol['errors'], "
+            "global_mean=ol['global_mean'], count=ol['count'])") % ROOT
     with tempfile.TemporaryDirectory() as td:
         outs = []
         for host_min in ("1", str(1 << 40)):
             f = os.path.join(td, f"o{len(outs)}.npz")
             subprocess.run([sys.executable, "-c", code, f], check=True, env=dict(os.environ, BSFM_BA_MASK_HOST_MIN=host_min, BSFM_BA_MASK_THREADS="3"))
             outs.append(np.load(f))
-    for key in ("info", "R", "c", "f", "k", "pts"):
-        assert np.array_equal(outs[0][key], outs[1][key]), key
+    for key in ("info", "R", "c", "f", "k", "pts", "dist", "stats", "outliers", "errors", "global_mean", "count"):
+        assert np.array_equal(outs[0][key], outs[1][key], equal_nan=key == "stats"), key   # an empty camera's mean is NaN
 
 
 @pytest.mark.parametrize("n", [97, 450, 640])
