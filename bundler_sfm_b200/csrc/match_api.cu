@@ -380,6 +380,9 @@ static int64_t match_run_impl(bsfm_keydb *db, int img_begin, int img_end, int wi
     P.test_mode = test_mode;
     P.ratio = ratio;
     P.ratio_sq = (test_mode == 0) ? ratio * ratio : ratio * ratio * (1.0 + 1e-9);
+    // whether d0 == d1 > 0 passes the final test (the kernels' ratio_pass): at ratio 1.0 in test mode 1, as in the symmetric
+    // pass of bundler --add_images, the choice among keys tied for the nearest distance becomes part of the output
+    P.ties_pass = (test_mode == 0) ? (ratio * ratio > 1.0) : (ratio >= 1.0);
     P.neg2 = -2;
     P.cand = (int32_t *) (S + o_cand); P.cand_cap = (int32_t) cap;
     P.hard = (int32_t *) (S + o_hard);

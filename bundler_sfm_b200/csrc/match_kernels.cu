@@ -60,11 +60,15 @@ __global__ void prep_kernel(const uint8_t *__restrict__ raw, const int64_t *__re
 // implementation used to cross-check the tensor-core kernel at full size and as the selectable
 // BSFM_MATCH_KERNEL_DP4A path.  Exact top-2 with index per row; emits final matches directly.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void top2_insert(int &m1, int &m2, int &mi, int t, int idx)
+__device__ __forceinline__ void top2_insert(int &m1, int &m2, int &mi, int t, int idx, bool ties, const int32_t *perm_img)
 {
-    // keeps (m1 <= m2); first-seen wins ties (pr_queue_k.h:102-117 strict '>')
+    // keeps (m1 <= m2); a thread sees its columns in ascending norm-sorted position, so without `ties` the first seen wins a
+    // tie.  With `ties` (a tie can pass the ratio test) a tied column replaces the best when its caller index is smaller.
     if (t < m1) { m2 = m1; m1 = t; mi = idx; }
-    else if (t < m2) { m2 = t; }
+    else {
+        if (t < m2) m2 = t;
+        if (ties && t == m1 && perm_img[idx] < perm_img[mi]) mi = idx;
+    }
 }
 
 __global__ void __launch_bounds__(256) match_dp4a_kernel(MatchParams P)
@@ -79,6 +83,8 @@ __global__ void __launch_bounds__(256) match_dp4a_kernel(MatchParams P)
     const RunImage R = P.run_imgs[k];
     const int64_t a_row0 = (int64_t) (R.atile0 + (u - R.unit0)) * TILE_Q;
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const bool ties = P.ties_pass != 0;
+    const int32_t *perm_img = P.perm + R.db_row0;   // norm-sorted position of image R -> caller index
 
     // query tile -> sQ[k4][row]
     for (int idx = tid; idx < TILE_Q * 8; idx += 256) {
@@ -127,12 +133,13 @@ __global__ void __launch_bounds__(256) match_dp4a_kernel(MatchParams P)
 #pragma unroll
             for (int a = 0; a < 8; a++) {
                 int t = nb - 2 * (int) acc[a][b];
-                top2_insert(m1[a], m2[a], mi[a], t, col);
+                top2_insert(m1[a], m2[a], mi[a], t, col, ties, perm_img);
             }
         }
     }
 
-    // merge the 16 column-threads of every row (lanes differing in the low 4 bits)
+    // merge the 16 column-threads of every row (lanes differing in the low 4 bits); of two tied bests the smaller caller
+    // index wins, so the result does not depend on the shuffle tree
 #pragma unroll
     for (int a = 0; a < 8; a++) {
 #pragma unroll
@@ -142,7 +149,7 @@ __global__ void __launch_bounds__(256) match_dp4a_kernel(MatchParams P)
             int oi = __shfl_xor_sync(0xffffffffu, mi[a], o);
             int hi = max(m1[a], o1);
             int lo2 = min(m2[a], o2);
-            if (o1 < m1[a]) mi[a] = oi;
+            if (o1 < m1[a] || (o1 == m1[a] && perm_img[oi] < perm_img[mi[a]])) mi[a] = oi;
             m1[a] = min(m1[a], o1);
             m2[a] = min(hi, lo2);
         }
@@ -527,37 +534,43 @@ __global__ void __launch_bounds__(256) match_verify_kernel(MatchParams P, int nc
     const int f5 = P.cand[5 * cap + w];
     const int f6 = P.cand[6 * cap + w];
 
-    // up to 64 rows per candidate (bound chunks may be 64 wide): two distances per lane, lane-local top-2 first
-    int m1 = INT_MAX, m2 = INT_MAX, mi = lane;
-    if (lane < nvalid) m1 = sqdist_rows(P.keys_sw, qrow, (int64_t) db0 + lane);
+    // up to 64 rows per candidate (bound chunks may be 64 wide): two distances per lane, lane-local top-2 first.
+    // (m1, mk) orders by distance, then by caller index: of keys tied for the nearest distance the smallest caller index wins
+    int m1 = INT_MAX, m2 = INT_MAX, mi = lane, mk = INT_MAX;
+    if (lane < nvalid) { m1 = sqdist_rows(P.keys_sw, qrow, (int64_t) db0 + lane); mk = P.perm[db0 + lane]; }
     if (lane + 32 < nvalid) {
         const int d = sqdist_rows(P.keys_sw, qrow, (int64_t) db0 + lane + 32);
-        if (d < m1) { m2 = m1; m1 = d; mi = lane + 32; } else m2 = d;
+        const int k = P.perm[db0 + lane + 32];
+        if (d < m1 || (d == m1 && k < mk)) { m2 = m1; m1 = d; mi = lane + 32; mk = k; } else m2 = d;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         int o1 = __shfl_xor_sync(0xffffffffu, m1, o);
         int o2 = __shfl_xor_sync(0xffffffffu, m2, o);
         int oi = __shfl_xor_sync(0xffffffffu, mi, o);
+        int ok = __shfl_xor_sync(0xffffffffu, mk, o);
         int hi = max(m1, o1);
         int lo2 = min(m2, o2);
-        if (o1 < m1 || (o1 == m1 && oi < mi)) mi = oi;
+        if (o1 < m1 || (o1 == m1 && ok < mk)) { mi = oi; mk = ok; }
         m1 = min(m1, o1);
         m2 = min(hi, lo2);
     }
     if (lane == 0) {
         bool match = false, hard = false;
         if (f6 == INT_MIN) {
-            // exact mode: d0 = m1 is the global minimum, f5 bounds d1 from above through the other chunks
+            // exact mode: d0 = m1 is the global minimum, f5 bounds d1 from above through the other chunks.  f5 == m1 means
+            // another chunk holds a key at distance d0: when such a tie can pass, the full scan picks among all tied keys
             const int d1 = min(f5, m2);
-            match = ratio_pass(P, m1, d1);
+            if (P.ties_pass && f5 == m1) hard = true;
+            else match = ratio_pass(P, m1, d1);
         } else {
             // bound mode: the chunk with the smallest lower bound was recomputed exactly (m1, m2).  It holds the
             // global minimum iff m1 <= every other chunk's lower bound; d1 lies in [min(m2, L2), min(m2, Uo)].
+            // m1 == L2 leaves open a key of another chunk at distance d0: undecided when such a tie can pass
             const int na = P.norms[qrow];
             const int l2d = (f5 >= NORM_PAD_HALF) ? INT_MAX : na + f5;
             const int uod = (f6 >= NORM_PAD_HALF) ? INT_MAX : na + f6;
-            if (m1 > l2d) hard = true;
+            if (m1 > l2d || (P.ties_pass && m1 == l2d)) hard = true;
             else {
                 const int d1_low = min(m2, l2d), d1_up = min(m2, uod);
                 if (ratio_pass(P, m1, d1_low)) match = true;
@@ -590,7 +603,7 @@ __global__ void __launch_bounds__(256) match_verify_kernel(MatchParams P, int nc
 __global__ void __launch_bounds__(256) match_fullscan_kernel(MatchParams P, int nhard)
 {
     // one 256-thread block per hard row: every warp scans a strided eighth of the image, then the warps' top-2 merge
-    __shared__ int s_m1[8], s_m2[8], s_mi[8];
+    __shared__ int s_m1[8], s_m2[8], s_mi[8], s_mk[8];
     const int w = blockIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (w >= nhard) return;
@@ -598,16 +611,17 @@ __global__ void __launch_bounds__(256) match_fullscan_kernel(MatchParams P, int 
     const int qrow = P.hard[(size_t) P.cand_cap + w];
     const int u = P.unit_begin + (slot >> 7);
     const RunImage R = P.run_imgs[find_run_image(P.run_imgs, P.num_run_imgs, u)];
-    int m1 = INT_MAX, m2 = INT_MAX, mi = INT_MAX;
+    // (m1, mk) orders by distance, then by caller index: of keys tied for the nearest distance the smallest caller index wins
+    int m1 = INT_MAX, m2 = INT_MAX, mi = INT_MAX, mk = INT_MAX;
     for (int c = threadIdx.x; c < R.n; c += 256) {
         const int d = sqdist_rows(P.keys_sw, qrow, (int64_t) R.db_row0 + c);
-        if (d < m1) { m2 = m1; m1 = d; mi = c; } else if (d < m2) m2 = d;
+        const int k = P.perm[(int64_t) R.db_row0 + c];
+        if (d < m1 || (d == m1 && k < mk)) { m2 = m1; m1 = d; mi = c; mk = k; } else if (d < m2) m2 = d;
     }
-    // (value, index) top-2 merge; ties keep the smaller index (any tie of the two best fails the ratio test anyway)
-    auto merge = [&](int o1, int o2, int oi) {
+    auto merge = [&](int o1, int o2, int oi, int ok) {
         const int hi = max(m1, o1);
         const int lo2 = min(m2, o2);
-        if (o1 < m1 || (o1 == m1 && oi < mi)) mi = oi;
+        if (o1 < m1 || (o1 == m1 && ok < mk)) { mi = oi; mk = ok; }
         m1 = min(m1, o1);
         m2 = min(hi, lo2);
     };
@@ -616,12 +630,13 @@ __global__ void __launch_bounds__(256) match_fullscan_kernel(MatchParams P, int 
         const int o1 = __shfl_xor_sync(0xffffffffu, m1, o);
         const int o2 = __shfl_xor_sync(0xffffffffu, m2, o);
         const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
-        merge(o1, o2, oi);
+        const int ok = __shfl_xor_sync(0xffffffffu, mk, o);
+        merge(o1, o2, oi, ok);
     }
-    if (lane == 0) { s_m1[warp] = m1; s_m2[warp] = m2; s_mi[warp] = mi; }
+    if (lane == 0) { s_m1[warp] = m1; s_m2[warp] = m2; s_mi[warp] = mi; s_mk[warp] = mk; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        for (int q = 1; q < 8; q++) merge(s_m1[q], s_m2[q], s_mi[q]);
+        for (int q = 1; q < 8; q++) merge(s_m1[q], s_m2[q], s_mi[q], s_mk[q]);
         if (ratio_pass(P, m1, m2)) {
             int pos = atomicAdd(&P.counters[1], 1);
             if (pos < P.match_cap) { P.match_slot[pos] = match_sort_key(P, R, qrow); P.match_idx2[pos] = mi; }

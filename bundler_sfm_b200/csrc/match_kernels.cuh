@@ -75,6 +75,9 @@ struct MatchParams {
     double ratio;               // the ratio itself (test mode 1)
     int32_t test_mode;          // 0: (double) d0 < ratio^2 (double) d1          MatchKeys of keys2a.cpp:362 / :412
                                 // 1: sqrt((double) d0 / (double) d1) <= ratio   MatchKeys of keys.cpp:786 (bundler --add_images)
+    int32_t ties_pass;          // 1 iff d0 == d1 > 0 passes the ratio test (test mode 0 with ratio^2 > 1, test mode 1 with ratio >= 1):
+                                // only then is it observable which of several keys tied for the nearest distance is returned.
+                                // The rule is the smallest caller index (perm[]) among them, on every kernel.
     int32_t neg2;               // the constant -2 as a runtime value (see the epilogue of match_tc_kernel)
     int32_t epi_mode;           // 1 = bound epilogue (max tree on norm-sorted chunks), 0 = exact chunk minima
     // candidate list (tensor-core kernel): SoA int32 [7][cand_cap]: slot, qrow, db0, col0, nvalid, f5, f6

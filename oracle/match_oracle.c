@@ -14,8 +14,13 @@
  * from /root/reference, exact mode max_pts_visit=0) by tests/test_oracle_match.py, and against
  * the committed vectors in tests/golden/match_*.npz which that reference produced.
  *
- * Tie note: when two database keys tie for the best distance, d0==d1 and the ratio test cannot
- * pass for ratio<=1 (KeyMatchFull hard-codes 0.6), so index tie-breaking is unobservable.
+ * Tie note: when two database keys tie for the best distance, d0==d1.  The keys2a test cannot
+ * pass then for ratio<=1 (KeyMatchFull hard-codes 0.6), so which tied key wins is unobservable.
+ * The keys.cpp test sqrt(d0/d1) <= ratio passes it at ratio 1.0, which the symmetric pass of
+ * bundler --add_images uses (Bundle.cpp:3817-3820), so there the tied key is part of the output.
+ * This port returns the smallest caller index among the tied keys (first seen), and so does every
+ * GPU kernel.  The unmodified kd-tree returns the first tied key it visits, which can be another
+ * (tests/golden/match_ties_golden.npz records where).
  */
 #include <limits.h>
 #include <math.h>

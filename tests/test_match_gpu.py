@@ -102,13 +102,29 @@ def test_sharded_runs_concatenate(kernel, oracle):
     assert np.array_equal(np.concatenate(parts_m), m_all)
 
 
-def test_chunked_launches_equal_single_launch(kernel, monkeypatch):
-    sizes = [900, 800, 1000, 700]
+def test_chunked_launches_equal_single_launch(kernel, monkeypatch, oracle):
+    # 50 images of 1100 keys (10 units of 128 padded rows each): image i has 10 i units, 12 250 in all.  The default chunk
+    # (32 Mi query rows) takes them in one search; BSFM_MATCH_CHUNK_MSLOTS=1 (8192 units) needs two
+    sizes = [1100] * 50
     imgs = synth.sift_like_descriptors(len(sizes), sizes, seed=9)
-    ref = keymatch.key_match_full(imgs, -1, 0.6)
-    monkeypatch.setenv("BSFM_MATCH_CHUNK_MSLOTS", "1")   # 1 Mi slots/launch; forces several launches? (small here)
-    got = keymatch.key_match_full(imgs, -1, 0.6)
-    assert np.array_equal(ref[1], got[1]) and np.array_equal(ref[2], got[2])
+    keys, key_off = keymatch.concat_keys(imgs)
+    db = keymatch.KeyDatabase(keys, key_off)
+    try:
+        db.run(0, len(sizes), -1, 0.6)
+        ref, launches_ref = db.fetch(), db.timing()["launches"]
+        monkeypatch.setenv("BSFM_MATCH_CHUNK_MSLOTS", "1")
+        db.run(0, len(sizes), -1, 0.6)
+        got, launches = db.fetch(), db.timing()["launches"]
+    finally:
+        db.close()
+    assert np.array_equal(ref[0], got[0]) and np.array_equal(ref[1], got[1])
+    assert launches > launches_ref, (launches_ref, launches)
+    pairs = keymatch.pair_list(len(sizes))
+    starts = np.concatenate([[0], np.cumsum(got[0])])
+    picked = np.random.default_rng(3).choice(len(pairs), 30, replace=False)
+    for q in picked:
+        j, i = pairs[q]
+        assert np.array_equal(got[1][starts[q]:starts[q + 1]], oracle.match_pair_port(imgs[j], imgs[i], 0.6)), (j, i)
 
 
 def test_tc_equals_dp4a_at_scale(monkeypatch):
