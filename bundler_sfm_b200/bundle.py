@@ -70,15 +70,45 @@ def _bind_run_sfm(fn):
     return fn
 
 
+def _visibility_args(scene):
+    """the visibility arguments of a scene dict for the C entries -> (n, m, args, keep-alive).  A dense scene passes
+    [vmask] (n x m); a CRS scene (synth.crs_scene) passes [vis_ptr, vis_cam, nvis] to the _crs entries, with n = len(pts)
+    and m = len(R).  vis_ptr / vis_cam may be numpy arrays or int32 torch tensors (pageable, pinned or CUDA memory: their
+    own pointers are passed); an optional "nvis" entry declares a count other than len(vis_cam)."""
+    if "vis_ptr" not in scene:
+        vmask = np.ascontiguousarray(scene["vmask"], dtype=np.int8)
+        n, m = vmask.shape
+        return n, m, [vmask.ctypes.data], [vmask]
+    ptrs, keep = [], []
+    for key in ("vis_ptr", "vis_cam"):
+        a = scene[key]
+        if hasattr(a, "data_ptr"):
+            assert str(a.dtype) == "torch.int32" and a.is_contiguous(), key
+            ptrs.append(a.data_ptr() or None)
+        else:
+            a = np.ascontiguousarray(a, dtype=np.int32)
+            ptrs.append(a.ctypes.data)
+        keep.append(a)
+    nvis = int(scene.get("nvis", len(scene["vis_cam"])))
+    return len(scene["pts"]), len(scene["R"]), ptrs + [nvis], keep
+
+
+def observations(scene):
+    """(point, camera) of every observation of a dense or CRS scene, in the order of `projections`"""
+    if "vis_ptr" in scene:
+        ptr = np.asarray(scene["vis_ptr"], dtype=np.int64)
+        return np.repeat(np.arange(len(ptr) - 1), np.diff(ptr)), np.asarray(scene["vis_cam"], dtype=np.int64)
+    return np.nonzero(scene["vmask"])
+
+
 def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_centers=1, ncons=0, eps2=1e-12,
                  use_constraints=0, constrained=None, constraints=None, weights=None,
                  use_point_constraints=0, points_constraints=None, point_constraint_weight=0.0,
                  extra_info=False, export=False, fix_points=0, known=None, K_known=None, k_known=None):
-    """Calls a run_sfm-shaped C function (ours or the reference's) on a scene dict (synth.ba_scene).
-    known / K_known / k_known: calibrated cameras (see make_cameras).
+    """Calls a run_sfm-shaped C function (ours or the reference's) on a scene dict (synth.ba_scene), or
+    bsfm_run_sfm_crs on a CRS scene (synth.crs_scene).  known / K_known / k_known: calibrated cameras (see make_cameras).
     Returns a dict with the refined R, c, f, k, pts (+ info when the callee provides it)."""
-    vmask = np.ascontiguousarray(scene["vmask"], dtype=np.int8)
-    n, m = vmask.shape
+    n, m, vis_args, _keep = _visibility_args(scene)
     proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
     cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], constrained, constraints, weights, known, K_known, k_known)
     pts = np.ascontiguousarray(scene["pts"], dtype=np.float64).copy()
@@ -90,7 +120,7 @@ def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_cen
     export_keys = "VSUW" if export is True else (export or "")
     if export:   # Vout, Sout, Uout, Wout (sba_levmar.c:1633-2026)
         ex = {"V": np.zeros((n, 9)), "S": np.zeros((m * cnp, m * cnp)), "U": np.zeros((m, cnp * cnp)), "W": np.zeros((m * cnp, 3 * n))}
-    args = [n, m, ncons, vmask.ctypes.data, proj.ctypes.data, est_focal_length, 0, undistort, explicit_camera_centers,
+    args = [n, m, ncons, *vis_args, proj.ctypes.data, est_focal_length, 0, undistort, explicit_camera_centers,
             ctypes.addressof(cams), pts.ctypes.data, use_constraints, use_point_constraints,
             pc.ctypes.data if pc is not None else None, float(point_constraint_weight), int(fix_points), 0, float(eps2),
             ex["V"].ctypes.data if export and "V" in export_keys else None, ex["S"].ctypes.data if export and "S" in export_keys else None,
@@ -104,22 +134,24 @@ def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_cen
     return {"rc": rc, "R": R, "c": c, "f": f, "k": k, "pts": pts, "info": info, **ex}
 
 
-_run_sfm = None
+_run_sfm = {}
 
 
 def run_sfm(scene, **kw):
-    """GPU run_sfm (bsfm_run_sfm).  Raises on BSFM errors; returns the refined scene + info[10].
-    Keywords are those of call_run_sfm (known / K_known / k_known for calibrated cameras)."""
-    global _run_sfm
-    lib = load_library()
-    if _run_sfm is None:
-        fn = lib.bsfm_run_sfm
+    """GPU run_sfm: bsfm_run_sfm, or bsfm_run_sfm_crs for a scene with vis_ptr / vis_cam instead of vmask.  Raises on BSFM
+    errors; returns the refined scene + info[10].  Keywords are those of call_run_sfm (known / K_known / k_known for
+    calibrated cameras)."""
+    name = "bsfm_run_sfm_crs" if "vis_ptr" in scene else "bsfm_run_sfm"
+    if name not in _run_sfm:
+        fn = getattr(load_library(), name)
         _bind_run_sfm(fn)
+        if name.endswith("_crs"):   # vmask -> vis_ptr, vis_cam, nvis
+            fn.argtypes = fn.argtypes[:3] + [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + fn.argtypes[4:]
         fn.argtypes = fn.argtypes + [ctypes.c_void_p]
         fn.restype = ctypes.c_int
-        _run_sfm = fn
-    out = call_run_sfm(_run_sfm, scene, extra_info=True, **kw)
-    check(out["rc"], "bsfm_run_sfm")
+        _run_sfm[name] = fn
+    out = call_run_sfm(_run_sfm[name], scene, extra_info=True, **kw)
+    check(out["rc"], name)
     return out
 
 
@@ -153,9 +185,8 @@ def project_known(Pc, K_known, k_known):
 def reprojection_rmse(scene, sol, known=None, K_known=None, k_known=None):
     """sqrt(mean squared reprojection error) of a solution under the Bundler camera model
     (lib/sfm-driver/sfm.c:302-380), computed in numpy -- a test/bench metric, not a product path.
-    known / K_known / k_known: calibrated cameras, as for run_sfm."""
-    vmask = scene["vmask"]
-    pi, cj = np.nonzero(vmask)
+    known / K_known / k_known: calibrated cameras, as for run_sfm.  Dense or CRS scenes."""
+    pi, cj = observations(scene)
     R = sol["R"].reshape(-1, 3, 3)
     Pc = np.einsum("oij,oj->oi", R[cj], sol["pts"][pi] - sol["c"][cj])
     f = sol["f"][cj]
@@ -287,17 +318,20 @@ def mot_levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, points_ptr, cnp, R_init, f_f
 def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thresh=16.0, pt_protected=None, cap=None,
                           known=None, K_known=None, k_known=None):
     """bsfm_reprojection_outliers: the statistics / outlier pass BundlerApp::RunSFM_SBA runs after every run_sfm
-    (src/Bundle.cpp:659-856) on a scene dict (vmask, projections, R, c, f, k, pts).  Defaults are bundler's
+    (src/Bundle.cpp:659-856) on a scene dict (vmask, projections, R, c, f, k, pts), or bsfm_reprojection_outliers_crs on a
+    CRS scene (vis_ptr / vis_cam instead of vmask, see synth.crs_scene).  Defaults are bundler's
     m_min/max_proj_error_threshold (BundlerApp.h).  Returns dist[nvis], stats[m x 5] (n, mean, median, med80, thresh),
     outliers, errors, global_mean.  known / K_known / k_known: calibrated cameras, as for run_sfm."""
     lib = load_library()
-    fn = lib.bsfm_reprojection_outliers
+    crs = "vis_ptr" in scene
+    name = "bsfm_reprojection_outliers_crs" if crs else "bsfm_reprojection_outliers"
+    fn = getattr(lib, name)
     fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+    vis_types = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] if crs else [ctypes.c_void_p]
+    fn.argtypes = [ctypes.c_int, ctypes.c_int] + vis_types + [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                    ctypes.c_double, ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                    ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
-    vmask = np.ascontiguousarray(scene["vmask"], dtype=np.int8)
-    n, m = vmask.shape
+    n, m, vis_args, _keep = _visibility_args(scene)
     proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
     cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], known=known, K_known=K_known, k_known=k_known)
     pts = np.ascontiguousarray(scene["pts"], dtype=np.float64)
@@ -307,9 +341,9 @@ def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thre
     stats = np.zeros((m, 5)); dist = np.zeros(nvis)
     out_idx = np.zeros(max(cap, 1), np.int32); out_err = np.zeros(max(cap, 1))
     gm = ctypes.c_double()
-    rc = fn(n, m, vmask.ctypes.data, proj.ctypes.data, ctypes.addressof(cams), pts.ctypes.data, int(estimate_distortion),
+    rc = fn(n, m, *vis_args, proj.ctypes.data, ctypes.addressof(cams), pts.ctypes.data, int(estimate_distortion),
             float(min_thresh), float(max_thresh), None if prot is None else prot.ctypes.data, stats.ctypes.data, dist.ctypes.data,
             out_idx.ctypes.data, out_err.ctypes.data, cap, ctypes.byref(gm))
-    check(rc, "bsfm_reprojection_outliers")
+    check(rc, name)
     k = min(rc, cap)
     return {"dist": dist, "stats": stats, "outliers": out_idx[:k].copy(), "errors": out_err[:k].copy(), "global_mean": gm.value, "count": rc}

@@ -110,16 +110,17 @@ __global__ void outlier_err_kernel(int nvis, const int *obs_cam, const int *obs_
 using namespace bsfm;
 using namespace bsfm::ba;
 
-extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const char *vmask, const double *projections,
-                                          const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion,
-                                          double min_proj_error_threshold, double max_proj_error_threshold,
-                                          const char *pt_protected, double *cam_stats, double *obs_dist,
-                                          int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
+// the outlier pass on either visibility source (bsfm_reprojection_outliers, bsfm_reprojection_outliers_crs)
+static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src, const double *projections,
+                         const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion,
+                         double min_proj_error_threshold, double max_proj_error_threshold,
+                         const char *pt_protected, double *cam_stats, double *obs_dist,
+                         int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
 {
     clear_error();
     { int rc = require_device(); if (rc != BSFM_OK) return rc; }
     const int n = num_pts, m = num_cameras;
-    if (n <= 0 || m <= 0 || !vmask || !projections || !cams || !pts || cap < 0 || (cap > 0 && (!outliers || !outlier_errors))) {
+    if (n <= 0 || m <= 0 || !vis_src.present() || !projections || !cams || !pts || cap < 0 || (cap > 0 && (!outliers || !outlier_errors))) {
         set_error("bsfm_reprojection_outliers: bad arguments");
         return BSFM_ERR_ARG;
     }
@@ -132,7 +133,7 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
     // the legacy default stream, as every copy below: callers may pass device pointers written on it
     DeviceArena D(0);
     Visibility vis;
-    TRY(build_visibility(vmask, n, m, 0, D, vis));
+    TRY(build_visibility(vis_src, n, m, 0, D, vis));
     const int nvis = vis.nvis;
     if (nvis <= 0) { set_error("bsfm_reprojection_outliers: empty visibility mask"); return BSFM_ERR_ARG; }
     int *d_obs_cam = vis.obs_cam, *d_obs_pt = vis.obs_pt, *d_cam_obs = vis.cam_obs, *d_cam_ptr = vis.cam_ptr;
@@ -196,4 +197,27 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
     const int total = (int) found.size();
     for (int q = 0; q < total && q < cap; q++) { outliers[q] = found[q].second; outlier_errors[q] = err[found[q].second]; }
     return total;
+}
+
+extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const char *vmask, const double *projections,
+                                          const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion,
+                                          double min_proj_error_threshold, double max_proj_error_threshold,
+                                          const char *pt_protected, double *cam_stats, double *obs_dist,
+                                          int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
+{
+    return outliers_impl(num_pts, num_cameras, VisSource::mask(vmask), projections, cams, pts, estimate_distortion,
+                         min_proj_error_threshold, max_proj_error_threshold, pt_protected, cam_stats, obs_dist, outliers,
+                         outlier_errors, cap, global_mean);
+}
+
+extern "C" int bsfm_reprojection_outliers_crs(int num_pts, int num_cameras, const int32_t *vis_ptr, const int32_t *vis_cam,
+                                              int nvis, const double *projections, const bsfm_camera_params_t *cams,
+                                              const bsfm_v3_t *pts, int estimate_distortion,
+                                              double min_proj_error_threshold, double max_proj_error_threshold,
+                                              const char *pt_protected, double *cam_stats, double *obs_dist,
+                                              int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
+{
+    return outliers_impl(num_pts, num_cameras, VisSource::crs(vis_ptr, vis_cam, nvis), projections, cams, pts,
+                         estimate_distortion, min_proj_error_threshold, max_proj_error_threshold, pt_protected, cam_stats,
+                         obs_dist, outliers, outlier_errors, cap, global_mean);
 }

@@ -1,9 +1,10 @@
-// ba_setup.cu -- setup of a BA call (ba_setup.h): device memory pool, visibility mask -> CRS and camera-major permutation,
+// ba_setup.cu -- setup of a BA call (ba_setup.h): device memory pool, visibility (mask or CRS) -> CRS and camera-major permutation,
 // Schur structure, and the kernels that build them.
 #include "ba_setup.h"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
+#include <climits>
 #include <cstdlib>
 #include <map>
 #include <mutex>
@@ -49,6 +50,37 @@ __global__ void csr_rows_kernel(const int *rowptr, int n, int *obs_pt)
     const int lane = threadIdx.x & 31;
     if (i >= n) return;
     for (int q = rowptr[i] + lane; q < rowptr[i + 1]; q += 32) obs_pt[q] = i;
+}
+
+// Why a caller's CRS is refused; for one point the lowest code is reported
+enum CrsFault { CRS_FIRST_PTR = 1, CRS_LAST_PTR, CRS_PTR_RANGE, CRS_PTR_DECREASES, CRS_CAM_RANGE, CRS_CAM_ORDER };
+
+// A caller's CRS, checked before anything else reads it, one warp per point; obs_pt is filled on the way.  The lowest
+// faulty point and its lowest fault go to *verdict as (point << 3 | fault) (left at ~0 when the CRS is sound).  Every
+// index is bounded before it is dereferenced: point i < n reads rowptr[i] and rowptr[i + 1] (n + 1 entries), and
+// obs_cam / obs_pt are touched only at q in [p0, p1) after 0 <= p0 <= p1 <= nvis has been established.
+__global__ void crs_check_kernel(const int *rowptr, const int *obs_cam, int n, int m, int nvis, int *obs_pt,
+                                 unsigned long long *verdict)
+{
+    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;
+    const int p0 = rowptr[i], p1 = rowptr[i + 1];
+    int fault = 0;
+    if (i == 0 && p0 != 0) fault = CRS_FIRST_PTR;
+    else if (i == n - 1 && p1 != nvis) fault = CRS_LAST_PTR;
+    else if (p0 < 0 || p1 > nvis) fault = CRS_PTR_RANGE;
+    else if (p1 < p0) fault = CRS_PTR_DECREASES;
+    if (fault) {
+        if (lane == 0) atomicMin(verdict, ((unsigned long long) i << 3) | fault);
+        return;
+    }
+    for (int q = p0 + lane; q < p1; q += 32) {
+        const int c = obs_cam[q];
+        fault = (c < 0 || c >= m) ? CRS_CAM_RANGE : (q > p0 && obs_cam[q - 1] >= c) ? CRS_CAM_ORDER : 0;
+        if (fault) atomicMin(verdict, ((unsigned long long) i << 3) | fault);
+        obs_pt[q] = i;
+    }
 }
 
 __global__ void iota_kernel(int *v, int count)
@@ -172,51 +204,99 @@ int DeviceArena::alloc_bytes(void **out, size_t bytes)
     return BSFM_OK;
 }
 
-// visibility: vmask -> CRS (sba_levmar.c:652-663), camera-major permutation
-int build_visibility(const char *vmask, int n, int m, cudaStream_t st, DeviceArena &D, Visibility &V)
+namespace {
+const char *crs_fault_text(int fault)
+{
+    switch (fault) {
+    case CRS_FIRST_PTR: return "vis_ptr[0] != 0";
+    case CRS_LAST_PTR: return "vis_ptr[num_pts] != nvis";
+    case CRS_PTR_RANGE: return "vis_ptr outside [0, nvis]";
+    case CRS_PTR_DECREASES: return "vis_ptr decreases";
+    case CRS_CAM_RANGE: return "camera index outside [0, num_cameras)";
+    default: return "cameras not strictly ascending";
+    }
+}
+}  // namespace
+
+// Visibility (idxij, sba_levmar.c:652-663) from one of three sources:
+//   1. a dense mask scanned on the device: count, cub scan, one sync for nvis, fill of obs_cam and obs_pt;
+//   2. a host-resident dense mask scanned on the host (host_scan_vmask, behind BSFM_BA_MASK_HOST_MIN);
+//   3. the caller's CRS, checked on the device (crs_check_kernel) with one sync for the verdict before anything reads it.
+// Sources 2 and 3 share the CRS upload, and all three the camera-major tail, so the same visibility gives the same arrays
+// whichever source it came from.
+int build_visibility(const VisSource &src, int n, int m, cudaStream_t st, DeviceArena &D, Visibility &V)
 {
     // host-resident masks of at least BSFM_BA_MASK_HOST_MIN bytes are scanned on the host and only their CRS form is uploaded
     // (host_scan_vmask, common.cpp).  OFF by default: at config 3 it cuts the H2D bytes per solve from 560 to 75 MB, but the scan
     // of the 500 MB mask costs host time, and whether it beats the PCIe copy from pinned memory depends on the host.
     static const size_t host_scan_min = []() { const char *e = getenv("BSFM_BA_MASK_HOST_MIN"); return e ? (size_t) atoll(e) : ~(size_t) 0; }();
     bool host_mask = false;
-    if ((size_t) n * m >= host_scan_min) {
+    if (src.vmask && (size_t) n * m >= host_scan_min) {
         cudaPointerAttributes pa;
-        if (cudaPointerGetAttributes(&pa, vmask) == cudaSuccess) host_mask = (pa.type == cudaMemoryTypeHost || pa.type == cudaMemoryTypeUnregistered);
+        if (cudaPointerGetAttributes(&pa, src.vmask) == cudaSuccess) host_mask = (pa.type == cudaMemoryTypeHost || pa.type == cudaMemoryTypeUnregistered);
         else cudaGetLastError();
     }
-    char *d_vmask = nullptr;
-    int *d_rowcnt;
-    std::vector<int> h_rowptr, h_obs_cam;
-    TRY(D.alloc(&d_rowcnt, (size_t) n + 1));
-    TRY(D.alloc(&V.rowptr, (size_t) n + 1));
-    if (host_mask) {
-        host_scan_vmask(vmask, n, m, h_rowptr, h_obs_cam);
-        BSFM_CUDA_TRY(cudaMemcpyAsync(V.rowptr, h_rowptr.data(), ((size_t) n + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-        V.nvis = h_rowptr[n];
-    } else {
-        TRY(D.upload(&d_vmask, vmask, (size_t) n * m));   // host or device pointer (UVA)
+    if (src.vmask && !host_mask) {   // source 1
+        char *d_vmask;
+        int *d_rowcnt;
+        TRY(D.alloc(&d_rowcnt, (size_t) n + 1));
+        TRY(D.alloc(&V.rowptr, (size_t) n + 1));
+        TRY(D.upload(&d_vmask, src.vmask, (size_t) n * m));   // host or device pointer (UVA)
         BSFM_CUDA_TRY(cudaMemsetAsync(d_rowcnt, 0, ((size_t) n + 1) * sizeof(int), st));
         vmask_count_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(d_vmask, n, m, d_rowcnt);
         BSFM_KERNEL_CHECK();
         TRY(D.cub(2, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, d_rowcnt, V.rowptr, n + 1, st); }));
         BSFM_CUDA_TRY(cudaMemcpyAsync(&V.nvis, V.rowptr + n, sizeof(int), cudaMemcpyDeviceToHost, st));
         BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+        if (V.nvis <= 0) return BSFM_OK;
+        TRY(D.alloc(&V.obs_cam, (size_t) V.nvis)); TRY(D.alloc(&V.obs_pt, (size_t) V.nvis));
+        vmask_fill_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(d_vmask, n, m, V.rowptr, V.obs_cam, V.obs_pt);
+        BSFM_KERNEL_CHECK();
+    } else {                         // sources 2 and 3: CRS arrays in host or device memory
+        std::vector<int> h_rowptr, h_obs_cam;
+        const int *rowptr = src.vis_ptr, *obs_cam = src.vis_cam;
+        if (host_mask) {
+            host_scan_vmask(src.vmask, n, m, h_rowptr, h_obs_cam);
+            rowptr = h_rowptr.data(); obs_cam = h_obs_cam.data();
+            V.nvis = h_rowptr[n];
+        } else {
+            if (src.nvis < 0 || src.nvis > INT_MAX / 2) {   // the solver counts 2 * nvis measurements in an int
+                set_error("malformed visibility (CRS): nvis = %d is outside [0, %d]", src.nvis, INT_MAX / 2);
+                return BSFM_ERR_ARG;
+            }
+            V.nvis = src.nvis;
+        }
+        TRY(D.alloc(&V.rowptr, (size_t) n + 1));
+        BSFM_CUDA_TRY(cudaMemcpyAsync(V.rowptr, rowptr, ((size_t) n + 1) * sizeof(int), cudaMemcpyDefault, st));
+        if (V.nvis > 0) {
+            TRY(D.alloc(&V.obs_cam, (size_t) V.nvis)); TRY(D.alloc(&V.obs_pt, (size_t) V.nvis));
+            BSFM_CUDA_TRY(cudaMemcpyAsync(V.obs_cam, obs_cam, (size_t) V.nvis * sizeof(int), cudaMemcpyDefault, st));
+        }
+        if (host_mask) {
+            if (V.nvis > 0) {
+                csr_rows_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(V.rowptr, n, V.obs_pt);
+                BSFM_KERNEL_CHECK();
+            }
+        } else {
+            unsigned long long *d_verdict, verdict = 0;
+            TRY(D.alloc(&d_verdict, 1));
+            BSFM_CUDA_TRY(cudaMemsetAsync(d_verdict, 0xff, sizeof(unsigned long long), st));
+            crs_check_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(V.rowptr, V.obs_cam, n, m, V.nvis, V.obs_pt, d_verdict);
+            BSFM_KERNEL_CHECK();
+            BSFM_CUDA_TRY(cudaMemcpyAsync(&verdict, d_verdict, sizeof verdict, cudaMemcpyDeviceToHost, st));
+            BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+            if (verdict != ~0ULL) {
+                set_error("malformed visibility (CRS) at point %d: %s", (int) (verdict >> 3), crs_fault_text((int) (verdict & 7)));
+                return BSFM_ERR_ARG;
+            }
+        }
     }
+    // the shared tail: camera-major permutation, a stable sort of observation ids by camera.  The int keys sort as they
+    // are: cub's signed-key transform flips bit 31 only, outside the sorted bits [0, bits).
     const int nvis = V.nvis;
     if (nvis <= 0) return BSFM_OK;
     int *d_iota, *d_cam_sorted;
-    TRY(D.alloc(&V.obs_cam, (size_t) nvis)); TRY(D.alloc(&V.obs_pt, (size_t) nvis));
     TRY(D.alloc(&V.cam_ptr, (size_t) m + 1)); TRY(D.alloc(&V.cam_obs, (size_t) nvis)); TRY(D.alloc(&d_iota, (size_t) nvis));
-    if (host_mask) {
-        BSFM_CUDA_TRY(cudaMemcpyAsync(V.obs_cam, h_obs_cam.data(), (size_t) nvis * sizeof(int), cudaMemcpyHostToDevice, st));
-        csr_rows_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(V.rowptr, n, V.obs_pt);
-    } else {
-        vmask_fill_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(d_vmask, n, m, V.rowptr, V.obs_cam, V.obs_pt);
-    }
-    BSFM_KERNEL_CHECK();
-    // camera-major permutation: stable sort of observation ids by camera.  The int keys sort as they are: cub's signed-key
-    // transform flips bit 31 only, outside the sorted bits [0, bits).
     TRY(D.alloc(&d_cam_sorted, (size_t) nvis));
     iota_kernel<<<(nvis + 255) / 256, 256, 0, st>>>(d_iota, nvis);
     BSFM_KERNEL_CHECK();

@@ -1,5 +1,5 @@
 // ba_setup.h -- host side of the BA setup, shared by the LM solver (ba_solver.cu) and the outlier pass (ba_outliers.cu):
-// pooled device memory, cub's two-phase calls, and the structures built once per call from the visibility mask.
+// pooled device memory, cub's two-phase calls, and the structures built once per call from the visibility.
 #pragma once
 #include <algorithm>
 #include <utility>
@@ -63,8 +63,24 @@ struct Visibility {
     int *cam_obs = nullptr;   // nvis, observation ids grouped by camera, ascending point within each camera
     int *cam_ptr = nullptr;   // m + 1: camera j's observations are cam_obs[cam_ptr[j] .. cam_ptr[j + 1])
 };
-// from the dense n x m mask of the reference interface, a host or device pointer; synchronises `st` once to learn nvis
-int build_visibility(const char *vmask, int n, int m, cudaStream_t st, DeviceArena &D, Visibility &V);
+// Where a call's visibility comes from: the dense n x m mask of the reference interface, or the caller's own CRS arrays
+// (the layout of Visibility::rowptr / obs_cam).  Host (pageable or pinned) or device pointers.
+struct VisSource {
+    const char *vmask = nullptr;
+    const int32_t *vis_ptr = nullptr;   // n + 1
+    const int32_t *vis_cam = nullptr;   // nvis
+    int nvis = 0;
+    static VisSource mask(const char *vmask) { VisSource s; s.vmask = vmask; return s; }
+    static VisSource crs(const int32_t *vis_ptr, const int32_t *vis_cam, int nvis)
+    {
+        VisSource s; s.vis_ptr = vis_ptr; s.vis_cam = vis_cam; s.nvis = nvis; return s;
+    }
+    bool present() const { return vmask || (vis_ptr && (vis_cam || nvis == 0)); }
+};
+// Visibility from either source.  Synchronises `st` at most once: to learn nvis of a mask scanned on the device, or to
+// read the verdict on a caller's CRS.  A malformed CRS returns BSFM_ERR_ARG naming the lowest offending point
+// (crs_check_kernel, ba_setup.cu); nothing but that check reads the caller's arrays before the verdict is known.
+int build_visibility(const VisSource &src, int n, int m, cudaStream_t st, DeviceArena &D, Visibility &V);
 
 // Schur structure of P's visibility: fills P.nblocks, blk_key, blk_start, tuples, nchunks, chunk_off and schur_part
 int build_schur_structure(Problem &P, cudaStream_t st, DeviceArena &D);

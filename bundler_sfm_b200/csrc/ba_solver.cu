@@ -131,7 +131,7 @@ struct Solve {
         P.nlm = mot ? m * cnp : P.nvars;
         P.Sdim = Sdim;
     }
-    int visibility(const char *vmask, const double *x);
+    int visibility(const VisSource &vis, const double *x);
     int upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, const double *p, const double *fixed_pts,
                int use_constraints, const bsfm_camera_constraints_t *constraints,
                int use_point_constraints, const bsfm_point_constraints_t *point_constraints);
@@ -174,11 +174,11 @@ struct Solve {
     }
 };
 
-// visibility mask -> CRS and the camera-major permutation (sba_levmar.c:652-663), measurements
-int Solve::visibility(const char *vmask, const double *x)
+// visibility -> CRS and the camera-major permutation (sba_levmar.c:652-663), measurements
+int Solve::visibility(const VisSource &vis, const double *x)
 {
     Visibility V;
-    TRY(build_visibility(vmask, n, m, st, D, V));
+    TRY(build_visibility(vis, n, m, st, D, V));
     nvis = V.nvis;
     P.nvis = nvis;
     nobs = nvis * 2;
@@ -426,7 +426,7 @@ int Solve::export_blocks(double *Vout, double *Sout, double *Uout, double *Wout)
 
 // Shared implementation of the two LM drivers (mot: see Solve).
 // init_params (nullable, m entries): the calibrated-camera fields (known_intrinsics, K_known, k_known) are read.
-static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
+static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon, const VisSource &vis, double *p, int cnp, int pnp,
                        const double *x, const double *covx, int mnp,
                        const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, int jac_mode,
                        int itmax, int verbose, const double opts[6], double info[10],
@@ -436,7 +436,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
 {
     clear_error();
     TRY(require_device());
-    if (n <= 0 || m <= 0 || mcon < 0 || mcon >= m || !vmask || !p || !x || !model || !opts || (mot && !fixed_pts)) {
+    if (n <= 0 || m <= 0 || mcon < 0 || mcon >= m || !vis.present() || !p || !x || !model || !opts || (mot && !fixed_pts)) {
         set_error("bsfm_sba_motstr_levmar_model: bad arguments (n=%d m=%d mcon=%d)", n, m, mcon);
         return BSFM_ERR_ARG;
     }
@@ -461,7 +461,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     Solve S(mot, n, m, mcon, cnp, model, jac_mode, *ctx);
 
     S.PT.begin(0);
-    TRY(S.visibility(vmask, x));
+    TRY(S.visibility(vis, x));
     TRY(build_schur_structure(S.P, st, S.D));
     TRY(S.upload(model, init_params, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints));
     S.PT.end();
@@ -494,7 +494,7 @@ extern "C" int bsfm_sba_motstr_levmar_model_ki(int n, int m, int mcon, const cha
                                                double *Vout, double *Sout, double *Uout, double *Wout,
                                                const bsfm_camera_params_t *init_params)
 {
-    return levmar_impl(0, nullptr, n, m, mcon, vmask, p, cnp, pnp, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
+    return levmar_impl(0, nullptr, n, m, mcon, VisSource::mask(vmask), p, cnp, pnp, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
                        use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout);
 }
 
@@ -518,7 +518,7 @@ extern "C" int bsfm_sba_mot_levmar_model_ki(int n, int m, int mcon, const char *
                                             int use_constraints, const bsfm_camera_constraints_t *constraints,
                                             const bsfm_camera_params_t *init_params)
 {
-    return levmar_impl(1, points, n, m, mcon, vmask, p, cnp, 3, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
+    return levmar_impl(1, points, n, m, mcon, VisSource::mask(vmask), p, cnp, 3, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
                        use_constraints, constraints, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
 }
 
@@ -592,19 +592,19 @@ extern "C" int bsfm_ba_last_timing(float ms[6], int *iterations, int *launches)
     return BSFM_OK;
 }
 
-// == run_sfm, lib/sfm-driver/sfm.c:592-1003
-extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask, double *projections,
-                            int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
-                            bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
-                            int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
-                            double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
-                            double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
+// == run_sfm, lib/sfm-driver/sfm.c:592-1003, on either visibility source (bsfm_run_sfm, bsfm_run_sfm_crs)
+static int run_sfm_impl(int num_pts, int num_cameras, int ncons, const VisSource &vis, double *projections,
+                        int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
+                        bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                        int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
+                        double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                        double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
 {
     clear_error();
     if (fix_points && (Vout || Sout || Uout || Wout)) { set_error("bsfm_run_sfm: fix_points=1 has no V/S/U/W export (nor has the reference, sfm.c:843-856)"); return BSFM_ERR_UNSUPPORTED; }
     if (optimize_for_fisheye) { set_error("bsfm_run_sfm: optimize_for_fisheye=1 is outside the GPU path"); return BSFM_ERR_UNSUPPORTED; }
     if (est_focal_length && const_focal_length) { set_error("bsfm_run_sfm: const_focal_length is not implemented (nor in the reference, sfm.c:518-521)"); return BSFM_ERR_UNSUPPORTED; }
-    if (num_pts <= 0 || num_cameras <= 0 || !vmask || !projections || !init_camera_params || !init_pts) {
+    if (num_pts <= 0 || num_cameras <= 0 || !vis.present() || !projections || !init_camera_params || !init_pts) {
         set_error("bsfm_run_sfm: bad arguments"); return BSFM_ERR_ARG;
     }
 
@@ -686,15 +686,15 @@ extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask
     const int verbosity = verb_env ? atoi(verb_env) : 3;          // VERBOSITY 3, MAX_ITERS 150 (sfm.c:814-815)
     int rc;
     if (fix_points)     // sfm.c:843-849: motion-only BA, the points come from init_pts and stay as they are
-        rc = bsfm_sba_mot_levmar_model_ki(num_pts, num_cameras, ncons, vmask, params.data(), cnp, projections, nullptr, 2,
-                                          &model, params.data() + num_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
-                                          use_constraints, use_constraints ? constraints.data() : nullptr, init_camera_params);
+        rc = levmar_impl(1, params.data() + num_camera_params, num_pts, num_cameras, ncons, vis, params.data(), cnp, 3, projections,
+                         nullptr, 2, &model, init_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                         use_constraints, use_constraints ? constraints.data() : nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
     else
-        rc = bsfm_sba_motstr_levmar_model_ki(num_pts, num_cameras, ncons, vmask, params.data(), cnp, 3, projections, nullptr, 2,
-                                             &model, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
-                                             use_constraints, use_constraints ? constraints.data() : nullptr,
-                                             use_point_constraints, use_point_constraints ? point_constraints.data() : nullptr,
-                                             Vout, Sout, Uout, Wout, init_camera_params);
+        rc = levmar_impl(0, nullptr, num_pts, num_cameras, ncons, vis, params.data(), cnp, 3, projections, nullptr, 2,
+                         &model, init_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                         use_constraints, use_constraints ? constraints.data() : nullptr,
+                         use_point_constraints, use_point_constraints ? point_constraints.data() : nullptr,
+                         Vout, Sout, Uout, Wout);
     if (rc < -1) {              // BSFM_ERR_*: nothing was solved; the caller's cameras get their scale fields back (they were set
         for (int j = 0; j < num_cameras; j++) { init_camera_params[j].f_scale = 1.0; init_camera_params[j].k_scale = 1.0; }   // to 0.001 / 5 above)
         return rc;
@@ -738,4 +738,29 @@ extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask
     for (int i = 0; i < num_pts; i++)
         for (int q = 0; q < 3; q++) init_pts[i].p[q] = params[(size_t) num_camera_params + 3 * (size_t) i + q];
     return BSFM_OK;
+}
+
+extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask, double *projections,
+                            int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
+                            bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                            int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
+                            double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                            double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
+{
+    return run_sfm_impl(num_pts, num_cameras, ncons, VisSource::mask(vmask), projections, est_focal_length, const_focal_length,
+                        undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints, use_point_constraints,
+                        pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2, Vout, Sout, Uout, Wout, info_out);
+}
+
+extern "C" int bsfm_run_sfm_crs(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                                double *projections, int est_focal_length, int const_focal_length, int undistort,
+                                int explicit_camera_centers, bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                                int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
+                                double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                                double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
+{
+    return run_sfm_impl(num_pts, num_cameras, ncons, VisSource::crs(vis_ptr, vis_cam, nvis), projections, est_focal_length,
+                        const_focal_length, undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints,
+                        use_point_constraints, pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2,
+                        Vout, Sout, Uout, Wout, info_out);
 }

@@ -144,6 +144,18 @@ def ba_scene_known_intrinsics(num_cameras=20, num_points=2000, views_per_point=5
     }
 
 
+def crs_scene(scene):
+    """a copy of a scene dict whose visibility is CRS instead of the dense vmask: vis_ptr [n+1] int32 (point i's
+    observations are vis_ptr[i]..vis_ptr[i+1]) and vis_cam [nvis] int32 (ascending camera within a point), i.e.
+    np.nonzero(vmask) in row-major order, the order of `projections`"""
+    vmask = np.asarray(scene["vmask"])
+    pi, cj = np.nonzero(vmask)
+    out = {k: v for k, v in scene.items() if k != "vmask"}
+    out["vis_ptr"] = np.concatenate([[0], np.cumsum(np.bincount(pi, minlength=vmask.shape[0]))]).astype(np.int32)
+    out["vis_cam"] = cj.astype(np.int32)
+    return out
+
+
 def ki_kwargs(scene):
     """the calibration keywords (known, K_known, k_known) of a scene for run_sfm / call_run_sfm / reprojection_rmse /
     reprojection_outliers; empty for a scene without calibrated cameras"""

@@ -140,6 +140,29 @@ int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask, double *p
                  double point_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
                  double *Vout, double *Sout, double *Uout, double *Wout, double *info_out);
 
+/* Visibility in CRS form, accepted by the _crs entries below in place of the dense num_pts x num_cameras vmask.  It is
+ * the layout sba builds from vmask itself (idxij, lib/sba-1.5/sba_levmar.c:652-663):
+ *   vis_ptr (num_pts + 1): point i's observations are [vis_ptr[i], vis_ptr[i + 1])
+ *   vis_cam (nvis):        the camera of each observation, strictly ascending within a point
+ * `projections` keep the order of the dense entries: point-major, ascending camera within a point, i.e. observation q
+ * of the CRS.  vis_ptr and vis_cam may be host (pageable or pinned) or device pointers, like vmask.  A vmask and the CRS
+ * of its non-zero bytes give bitwise identical results.  The arrays are checked on the device before anything reads
+ * them; the call returns BSFM_ERR_ARG, with a message naming the lowest offending point and the fault, when
+ *   nvis < 0 or 2 * nvis overflows int;  vis_ptr[0] != 0 (point 0);  vis_ptr[num_pts] != nvis (point num_pts - 1);
+ *   vis_ptr[i] or vis_ptr[i + 1] outside [0, nvis], or vis_ptr[i + 1] < vis_ptr[i] (point i);
+ *   a camera index outside [0, num_cameras), or cameras not strictly ascending, in point i's observations.
+ * For one point the faults are reported in this order.  vis_cam may be NULL when nvis == 0.                          */
+
+/* bsfm_run_sfm (run_sfm, lib/sfm-driver/sfm.c:592-1003) with the visibility as CRS: every other argument, return code,
+ * print and in/out rule is that of bsfm_run_sfm.  nvis == 0 returns SBA_ERROR (-1), "fewer measurements than
+ * unknowns", like an empty vmask.                                                                                 */
+int bsfm_run_sfm_crs(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                     double *projections, int est_focal_length, int const_focal_length, int undistort,
+                     int explicit_camera_centers, bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                     int use_constraints, int use_point_constraints, bsfm_v3_t *points_constraints,
+                     double point_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                     double *Vout, double *Sout, double *Uout, double *Wout, double *info_out);
+
 /* The reprojection statistics / outlier pass BundlerApp::RunSFM_SBA runs after every run_sfm on the same
  * vmask / projections / cameras / points (src/Bundle.cpp:659-856), as one call (SURVEY.md 8f row 1):
  *   dist(obs)   = || sfm_project_rd(camera, point, estimate_distortion, explicit centres) - measurement ||  (:721-754)
@@ -162,6 +185,15 @@ int bsfm_reprojection_outliers(int num_pts, int num_cameras, const char *vmask, 
                                double min_proj_error_threshold, double max_proj_error_threshold,
                                const char *pt_protected, double *cam_stats, double *obs_dist,
                                int32_t *outliers, double *outlier_errors, int cap, double *global_mean);
+
+/* bsfm_reprojection_outliers (src/Bundle.cpp:659-856) with the visibility as CRS (see bsfm_run_sfm_crs): every other
+ * argument and output is that of bsfm_reprojection_outliers.  nvis == 0 returns BSFM_ERR_ARG, "empty visibility",
+ * like an empty vmask.                                                                                           */
+int bsfm_reprojection_outliers_crs(int num_pts, int num_cameras, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                                   const double *projections, const bsfm_camera_params_t *cams, const bsfm_v3_t *pts,
+                                   int estimate_distortion, double min_proj_error_threshold, double max_proj_error_threshold,
+                                   const char *pt_protected, double *cam_stats, double *obs_dist,
+                                   int32_t *outliers, double *outlier_errors, int cap, double *global_mean);
 
 /* == sba_Axb_Chol (lib/sba-1.5/sba_lapack.c:374-485, called at sba_levmar.c:1343): x = A^-1 B for a symmetric
  * positive definite m x m matrix (dpotrf + dpotrs in the reference).  A, B, x: host or device pointers; A and B are
