@@ -170,7 +170,11 @@ constexpr int SY_CONSUMERS = 8, SY_THREADS = 32 * (SY_CONSUMERS + 4);      // tw
 // Registers: 168 per thread at launch (384 threads, one CTA per SM); the producer warpgroup gives 128 of them back and the
 // consumers take them: 4 warps x 40 + 8 warps x 232 = 12 warps x 168
 constexpr int SY_PRODUCER_REGS = 40, SY_CONSUMER_REGS = 232;
-constexpr size_t SY_SMEM = (size_t) SY_STAGES * 2 * SY_BLOCK * sizeof(double) + 2 * SY_STAGES * 8;
+// The shared list of a launch's nonzero row blocks: 16-bit entries behind two int counts.  A launch with more row blocks
+// (n > 16 K) keeps every tile.  The list is kept this short on purpose: the same kernel with 2 KB or 8 KB more shared memory
+// (even without the skip) returned wrong factors of dense systems from n ~ 3800 on (H100, cause not found, DESIGN.md §8).
+constexpr int SY_MAX_RB = 128;
+constexpr size_t SY_SMEM = (size_t) SY_STAGES * 2 * SY_BLOCK * sizeof(double) + 2 * SY_STAGES * 8 + 2 * sizeof(int) + SY_MAX_RB * sizeof(uint16_t);
 __device__ __forceinline__ size_t syrk_img_index(int q, int c)
 {
     const int r = q & (SY_BT - 1), k = c & (SY_BK - 1), t = k & 3;
@@ -187,6 +191,11 @@ static size_t syrk_img_doubles(int n) { return (size_t) ((n + 1 - LNBO + SY_BT -
 // [16 wr, +16) x [16 wc, +16) of the current 64 x 32 sub-block as 2 x 2 accumulator tiles.
 // Source rows: matrix rows of A below the diagonal block (ident == 0), or rows of the 256 x 256 identity (ident == 1:
 // the result is L_kk^-T, the inverse the back substitution multiplies with; blockIdx.y = panel).
+// ident == 0 also records one flag per CTA: SLAB_NONZERO when a value it wrote is != 0 (NaN included), SLAB_NONFINITE
+// when one is NaN or infinite.  A CTA whose source rows are all +-0 skips the solve and writes +0: what the solve returns
+// for them whenever the diagonal block factored (finite L_kk and Z).  Its image rows are written too: the trailing update
+// reads them when the other 64 rows of their 128-row block are nonzero.
+constexpr int SLAB_NONZERO = 1, SLAB_NONFINITE = 2;
 constexpr int TR_ROWS = 64;
 constexpr int TR_LDX = LNBO + 4;       // pitch = 4 (mod 16) doubles: conflict-free DMMA fragment loads
 constexpr int TR_LDB = LNB + 4;
@@ -196,6 +205,7 @@ struct TrsmArgs {
     const double *A;        // ident == 0: source rows (matrix, pitch ld)
     double *dst;            // destination rows: dst[(dst_row0 + r) * dst_ld + dst_col0 + c]
     double *img;            // ident == 0, not null: the rows also go to the panel image of the trailing update
+    int *flags;             // ident == 0: the panel's zero flags, flags[blockIdx.x] = SLAB_* bits of the rows this CTA wrote
     const double *Lfac;     // factor matrix (the panel's diagonal block is read from it)
     const double *linv_all;
     int ld, dst_ld, nrows, ident;
@@ -216,6 +226,7 @@ __global__ void __launch_bounds__(256) chol_trsm_kernel(const TrsmArgs T)
     if (rcount <= 0) return;
     const double *Lfac = T.Lfac;
     const int ld = T.ld;
+    bool src_nz = false;
     for (int r0 = 0; r0 < TR_ROWS; r0 += 32) {       // thread = column, 32 rows per batch: 32 independent loads in flight
         double v[32];
 #pragma unroll
@@ -225,9 +236,10 @@ __global__ void __launch_bounds__(256) chol_trsm_kernel(const TrsmArgs T)
             if (r < rcount && c < nb) v[i] = T.ident ? ((row0 + r == c) ? 1.0 : 0.0) : T.A[(size_t) (row0 + r) * ld + (k0 + c)];
         }
 #pragma unroll
-        for (int i = 0; i < 32; i++) Xs[(r0 + i) * TR_LDX + tid] = v[i];
+        for (int i = 0; i < 32; i++) { Xs[(r0 + i) * TR_LDX + tid] = v[i]; src_nz |= v[i] != 0.0; }
     }
-    const int nsub = (nb + LNB - 1) / LNB;
+    const bool src_zero = !T.ident && !__syncthreads_or(src_nz);
+    const int nsub = src_zero ? 0 : (nb + LNB - 1) / LNB;
     const int wr = warp & 3, wc = warp >> 2;
     const double *xrow0 = Xs + (wr * 16 + g) * TR_LDX, *xrow1 = xrow0 + 8 * TR_LDX;
     double pre[4 * TR_NLB];      // the blocks of the NEXT sub-step, 4 elements of each per thread
@@ -246,7 +258,7 @@ __global__ void __launch_bounds__(256) chol_trsm_kernel(const TrsmArgs T)
             }
         }
     };
-    trsm_prefetch(0);
+    if (nsub > 0) trsm_prefetch(0);
     __syncthreads();
     for (int s = 0; s < nsub; s++) {
         const int w = min(LNB, nb - s * LNB);
@@ -310,23 +322,36 @@ __global__ void __launch_bounds__(256) chol_trsm_kernel(const TrsmArgs T)
         }
     }
     __syncthreads();
+    int bits = 0;
     for (int e = tid; e < TR_ROWS * LNBO; e += 256) {
         const int rr = e >> 8, c = e & 255;
         if (rr < rcount && c < nb) {
             if (T.ident) T.dst[((size_t) blockIdx.y * LNBO + row0 + rr) * LNBO + c] = Xs[rr * TR_LDX + c];
             else {
-                T.dst[(size_t) (row0 + rr) * T.dst_ld + (k0 + c)] = Xs[rr * TR_LDX + c];
-                if (T.img) T.img[syrk_img_index((int) blockIdx.x * TR_ROWS + rr, c)] = Xs[rr * TR_LDX + c];
+                const double v = src_zero ? 0.0 : Xs[rr * TR_LDX + c];
+                bits |= (v != 0.0 ? SLAB_NONZERO : 0) | (isfinite(v) ? 0 : SLAB_NONFINITE);
+                T.dst[(size_t) (row0 + rr) * T.dst_ld + (k0 + c)] = v;
+                if (T.img) T.img[syrk_img_index((int) blockIdx.x * TR_ROWS + rr, c)] = v;
             }
         }
+    }
+    if (!T.ident) {
+        const int nz = __syncthreads_or(bits & SLAB_NONZERO), nf = __syncthreads_or(bits & SLAB_NONFINITE);
+        if (tid == 0) T.flags[blockIdx.x] = (nz ? SLAB_NONZERO : 0) | (nf ? SLAB_NONFINITE : 0);
     }
 }
 
 // ---- trailing update on the fp64 tensor cores (DMMA) -----------------------------------------------
 // A[r][c] -= sum_{t < 256} L[r][t] L[c][t]  for c in [cb, ce), r in [c, nrows), over the 128 x 128 tiles of the lower
 // triangle only.  PERSISTENT: one CTA per SM walks a static list of tiles (column block by column block; CTA b takes tiles
-// b, b + grid, ...), with no atomics and no split K, so the result does not depend on the grid.  WARP-SPECIALISED, 384
-// threads:
+// b, b + grid, ...), with no atomics and no split K, so the result does not depend on the grid.
+// ZERO BLOCKS SKIPPED: the reduced camera system couples only cameras that share points, and its factor keeps many
+// 128-row panel blocks at exactly +-0 in the early panels.  The prologue lists the launch's row blocks whose two 64-row slabs
+// of the panel solve are not both flagged zero, and the tiles are the lower triangle of that list (columns inside
+// [cb, ce)).  A skipped tile changes no bit: with one operand all +-0 every product is +-0, the accumulators stay +0, and
+// C - (+0) is C (-0 and NaN included).  That needs the other operand finite, so a launch with a non-finite panel value keeps
+// every tile, as does one with more row blocks than the list holds.  Once the factor is dense the list is 0, 1, 2, ... and the tiles are those of the dense triangle.
+// WARP-SPECIALISED, 384 threads:
 //   warp 8      producer (warps 9..11 only hand their registers to the consumers and leave): a K chunk (32) of one operand of one tile is ONE contiguous 32 KB cp.async.bulk out of the pre-tiled
 //               panel image (below) into a ring of SY_STAGES (A, B) stages with full / empty mbarriers.  It runs ahead across
 //               tiles, so the next tile's first chunks land while the consumers write the previous tile back, and when it
@@ -349,8 +374,9 @@ __device__ __forceinline__ void dmma_m16n8k8(double (&d)[4], const double (&a)[4
 struct SyrkArgs {
     double *A;              // the matrix being factored (pitch ld, nrows rows)
     const double *img;      // panel image; its row 0 is matrix row img_row0
-    int ld, nrows, cb, ce, img_row0;
-    int nrb, ntiles;        // row blocks of 128 from cb; lower-triangle tiles of the launch
+    const int *flags;       // the panel solve's flags, one per 64 image rows (nslab of them)
+    int ld, nrows, cb, ce, img_row0, nslab;
+    int nrb, ncb;           // row blocks of 128 from cb; column blocks of 128 in [cb, ce)
 };
 
 __global__ void __launch_bounds__(SY_THREADS, 1) chol_syrk_dmma_kernel(const SyrkArgs S)
@@ -359,18 +385,43 @@ __global__ void __launch_bounds__(SY_THREADS, 1) chol_syrk_dmma_kernel(const Syr
     extern __shared__ __align__(128) double ssm[];
     const uint32_t sbase = smem_u32(ssm);
     const uint32_t bar_full = sbase + (uint32_t) (SY_STAGES * 2 * SY_BLOCK * sizeof(double)), bar_empty = bar_full + 8 * SY_STAGES;
+    int *counts = reinterpret_cast<int *>(ssm + SY_STAGES * 2 * SY_BLOCK + 2 * SY_STAGES);      // kept row blocks, kept column blocks
+    uint16_t *list = reinterpret_cast<uint16_t *>(counts + 2);                                  // [SY_MAX_RB]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int s = 0; s < SY_STAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, SY_CONSUMERS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    if (warp == 0) {      // the row blocks with a nonzero panel block, ascending; how many of them are column blocks
+        int nk = S.nrb, nkc = S.ncb;      // every row block: more than the list holds, or a non-finite panel value
+        if (S.nrb <= SY_MAX_RB) {
+            const int rb0 = (S.cb - S.img_row0) / SY_BT;
+            int k = 0, kc = 0;
+            bool nonfinite = false;
+            for (int r0 = 0; r0 < S.nrb; r0 += 32) {
+                const int rb = r0 + lane, s = 2 * (rb0 + rb);
+                const int f = (rb < S.nrb) ? S.flags[s] | ((s + 1 < S.nslab) ? S.flags[s + 1] : 0) : 0;
+                nonfinite |= __any_sync(0xffffffffu, f & SLAB_NONFINITE);
+                const uint32_t m = __ballot_sync(0xffffffffu, f != 0);
+                if (f) list[k + __popc(m & ((1u << lane) - 1))] = rb;
+                k += __popc(m);
+                kc += __popc(m & __ballot_sync(0xffffffffu, rb < S.ncb));
+            }
+            if (!nonfinite) { nk = k; nkc = kc; }
+        }
+        if (lane == 0) { counts[0] = nk; counts[1] = nkc; }
+    }
     __syncthreads();
+    const int nk = counts[0], nkc = counts[1];
+    const bool all = nk == S.nrb;      // every row block kept: the list is 0, 1, 2, ... (or was not built)
+    const int ntiles = nkc * nk - nkc * (nkc - 1) / 2;
+    if ((int) blockIdx.x >= ntiles) return;      // no tile for this CTA: no mbarrier is ever waited on
     const bool vec2 = (S.ld & 1) == 0;      // 16-byte accesses to the output need an even pitch
-    // tile t of the launch -> (row block, column block), column block by column block over the lower triangle
+    // tile t of the launch -> (row block, column block), column block by column block over the lower triangle of the list
     auto tile_of = [&](int t, int &rb, int &cbk) {
         int c = 0;
-        while (t >= S.nrb - c) { t -= S.nrb - c; c++; }
-        cbk = c; rb = c + t;
+        while (t >= nk - c) { t -= nk - c; c++; }
+        cbk = all ? c : list[c]; rb = all ? c + t : list[c + t];
     };
 
     if (warp >= SY_CONSUMERS) {
@@ -380,7 +431,7 @@ __global__ void __launch_bounds__(SY_THREADS, 1) chol_syrk_dmma_kernel(const Syr
         uint64_t keep;      // the panel image is read by a whole column of tiles: keep it in L2
         asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
         uint32_t st = 0, ph = 0;
-        for (int t = blockIdx.x; t < S.ntiles; t += gridDim.x) {
+        for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
             int rb, cbk;
             tile_of(t, rb, cbk);
             const int r0 = S.cb + rb * SY_BT, c0 = S.cb + cbk * SY_BT;
@@ -427,7 +478,7 @@ __global__ void __launch_bounds__(SY_THREADS, 1) chol_syrk_dmma_kernel(const Syr
         }
     };
     uint32_t st = 0, ph = 0;
-    for (int t = blockIdx.x; t < S.ntiles; t += gridDim.x) {
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         double acc[4][4][4];
 #pragma unroll
         for (int i = 0; i < 4; i++)
@@ -487,15 +538,41 @@ __global__ void __launch_bounds__(SY_THREADS, 1) chol_syrk_dmma_kernel(const Syr
 }
 
 // A[r][c] -= L[r][k0 : k0 + 256] . L[c][k0 : k0 + 256] over the lower triangle of rows [cb, nrows) x columns [cb, ce), with
-// the panel read from its image (row 0 = matrix row img_row0 = k0 + 256); at most max_ctas persistent CTAs
-static void syrk_dmma(cudaStream_t st, double *A, const double *img, int ld, int nrows, int cb, int ce, int img_row0, int max_ctas)
+// the panel read from its image (row 0 = matrix row img_row0 = k0 + 256) and its flags; at most max_ctas persistent CTAs.
+// The grid is that of the dense triangle: how many tiles are kept is known only on the device.
+static void syrk_dmma(cudaStream_t st, double *A, const double *img, const int *flags, int nslab, int ld, int nrows, int cb, int ce,
+                      int img_row0, int max_ctas)
 {
     SyrkArgs S = {};
-    S.A = A; S.img = img; S.ld = ld; S.nrows = nrows; S.cb = cb; S.ce = ce; S.img_row0 = img_row0;
+    S.A = A; S.img = img; S.flags = flags; S.nslab = nslab; S.ld = ld; S.nrows = nrows; S.cb = cb; S.ce = ce; S.img_row0 = img_row0;
     S.nrb = (nrows - cb + SY_BT - 1) / SY_BT;
-    const int ncb = (ce - cb + SY_BT - 1) / SY_BT;      // <= nrb: ce <= n < nrows
-    S.ntiles = ncb * S.nrb - ncb * (ncb - 1) / 2;
-    chol_syrk_dmma_kernel<<<std::min(S.ntiles, max_ctas), SY_THREADS, SY_SMEM, st>>>(S);
+    S.ncb = (ce - cb + SY_BT - 1) / SY_BT;      // <= nrb: ce <= n < nrows
+    const int ntiles = S.ncb * S.nrb - S.ncb * (S.ncb - 1) / 2;
+    chol_syrk_dmma_kernel<<<std::min(ntiles, max_ctas), SY_THREADS, SY_SMEM, st>>>(S);
+}
+
+// The lower-triangle elements (right-hand-side row included) of the tiles chol_syrk_dmma_kernel keeps in that launch, from
+// the panel's flags read back to the host: the trailing update's executed FLOPs are 2 x 256 x this
+static double syrk_kept_elements(const int *flags, int nslab, int nrows, int cb, int ce, int img_row0)
+{
+    const int nrb = (nrows - cb + SY_BT - 1) / SY_BT, ncb = (ce - cb + SY_BT - 1) / SY_BT, rb0 = (cb - img_row0) / SY_BT;
+    std::vector<int> list;
+    bool nonfinite = false;
+    for (int rb = 0; rb < nrb; rb++) {
+        const int s = 2 * (rb0 + rb), f = flags[s] | ((s + 1 < nslab) ? flags[s + 1] : 0);
+        nonfinite |= (f & SLAB_NONFINITE) != 0;
+        if (f) list.push_back(rb);
+    }
+    if (nonfinite || nrb > SY_MAX_RB) { list.resize(nrb); for (int rb = 0; rb < nrb; rb++) list[rb] = rb; }
+    double el = 0.0;
+    for (size_t j = 0; j < list.size() && list[j] < ncb; j++) {
+        const int c0 = cb + list[j] * SY_BT, c1 = std::min(c0 + SY_BT, ce);
+        for (size_t i = j; i < list.size(); i++) {
+            const int r0 = cb + list[i] * SY_BT, r1 = std::min(r0 + SY_BT, nrows);
+            for (int c = c0; c < c1; c++) el += std::max(0, r1 - std::max(r0, c));
+        }
+    }
+    return el;
 }
 
 // ---- back substitution L^T x = y, one launch per outer panel (last to first) --------------------------------------
@@ -564,7 +641,9 @@ struct CholProfile {
     bool on = false;
     float ms[4] = {0, 0, 0, 0};          // diag, trsm, trailing update, back substitution
     int launches[4] = {0, 0, 0, 0};
-    double fp64_flops = 0.0;      // trailing update only
+    double fp64_flops = 0.0;      // trailing update only, the tiles it executed
+    struct Update { size_t flag_off; int nslab, cb, ce, img_row0; };
+    std::vector<Update> updates;  // the trailing-update launches of the factorisation in flight
     std::vector<cudaEvent_t> pool;
     size_t used = 0;
     struct Span { int cls; cudaEvent_t a, b; };
@@ -607,6 +686,14 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
     double *img = xinv_ws;
     if (syrk_img_doubles(n) > (size_t) ((n + LNBO - 1) / LNBO) * LNBO * LNBO || (reinterpret_cast<uintptr_t>(img) & 15) != 0) {
         set_error("chol_solve_large: the panel image does not fit the 16-byte aligned xinv workspace");
+        return BSFM_ERR_ARG;
+    }
+    // the zero flags of every panel solve (a stride of one flag per 64 rows of the whole matrix per panel) at the end of linv_ws
+    int *flags = reinterpret_cast<int *>(linv_ws + chol_large_flags_offset(n));
+    const size_t flag_stride = (size_t) (nrows + TR_ROWS - 1) / TR_ROWS;
+    if (chol_large_flags_offset(n) + (chol_large_flag_count(n) + 1) / 2 > chol_ws_doubles(n) ||
+        (size_t) ((n + LNBO - 1) / LNBO) * flag_stride > chol_large_flag_count(n)) {
+        set_error("chol_solve_large: the zero flags of n = %d do not fit the workspace", n);
         return BSFM_ERR_ARG;
     }
     // Look-ahead: the diagonal block of panel p+1 is a serial chain on ONE SM.  The trailing update of panel p is therefore
@@ -656,21 +743,24 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
         diag_done = false;
         const int rows_below = nrows - k1;     // >= 1: the right-hand side row
         g_prof.begin(1, st);
+        const int nslab = (rows_below + TR_ROWS - 1) / TR_ROWS;
+        const size_t flag_off = (size_t) (k0 / LNBO) * flag_stride;      // one flag array per panel: still readable after the factorisation
         TrsmArgs T = {};
         T.A = A; T.dst = Lmat; T.Lfac = Lmat; T.linv_all = linv_ws; T.ld = ld; T.dst_ld = ld; T.nrows = nrows; T.ident = 0; T.k0 = k0; T.nb = nb; T.n = n;
         T.img = (k1 < n) ? img : nullptr;      // k1 < n: a full 256-column panel with a trailing update
-        chol_trsm_kernel<<<(rows_below + TR_ROWS - 1) / TR_ROWS, 256, TR_SMEM_DOUBLES * sizeof(double), st>>>(T);
+        T.flags = flags + flag_off;
+        chol_trsm_kernel<<<nslab, 256, TR_SMEM_DOUBLES * sizeof(double), st>>>(T);
         BSFM_KERNEL_CHECK();
         g_prof.end(st);
         if (k1 < n) {
             g_prof.begin(2, st);
-            if (g_prof.on) {
-                const double tr = (double) (n - k1), pairs = tr * (tr + 1.0) * 0.5 + tr;     // lower triangle + right-hand side row
-                g_prof.fp64_flops += 2.0 * pairs * nb;
-            }
+            auto update = [&](int cb, int ce, int max_ctas) {
+                syrk_dmma(st, A, img, flags + flag_off, nslab, ld, nrows, cb, ce, k1, max_ctas);
+                if (g_prof.on) g_prof.updates.push_back({flag_off, nslab, cb, ce, k1});
+            };
             const int k2 = std::min(n, k1 + LNBO);      // the columns of panel p+1
             if (lookahead && k2 < n && !tail_fits(k1)) {
-                syrk_dmma(st, A, img, ld, nrows, k1, k2, k1, sms);
+                update(k1, k2, sms);
                 BSFM_KERNEL_CHECK();
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_col, st));
                 BSFM_CUDA_TRY(cudaStreamWaitEvent(side.st, side.e_col, 0));
@@ -679,9 +769,9 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_diag, side.st));
                 diag_done = true;
                 if (g_prof.on) g_prof.launches[0]++;
-                syrk_dmma(st, A, img, ld, nrows, k2, n, k1, sms - 1);
+                update(k2, n, sms - 1);
             } else {
-                syrk_dmma(st, A, img, ld, nrows, k1, n, k1, sms);
+                update(k1, n, sms);
             }
             BSFM_KERNEL_CHECK();
             g_prof.end(st);
@@ -704,7 +794,16 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
         BSFM_KERNEL_CHECK();
     }
     g_prof.end(st);
-    if (g_prof.on) g_prof.launches[3] += npan;     // end() counted one
+    if (g_prof.on) {
+        g_prof.launches[3] += npan;     // end() counted one
+        // the FLOPs of the tiles the trailing update executed: the flags are read back before the next factorisation reuses them
+        std::vector<int> hflags(chol_large_flag_count(n));
+        BSFM_CUDA_TRY(cudaMemcpyAsync(hflags.data(), flags, hflags.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+        for (const auto &u : g_prof.updates)
+            g_prof.fp64_flops += 2.0 * LNBO * syrk_kept_elements(hflags.data() + u.flag_off, u.nslab, nrows, u.cb, u.ce, u.img_row0);
+        g_prof.updates.clear();
+    }
     return BSFM_OK;
 }
 
@@ -717,6 +816,7 @@ extern "C" int bsfm_ba_chol_profile(int enable)
     g_prof.collect();
     for (int q = 0; q < 4; q++) { g_prof.ms[q] = 0; g_prof.launches[q] = 0; }
     g_prof.fp64_flops = 0.0;
+    g_prof.updates.clear();
     g_prof.on = enable != 0;
     return BSFM_OK;
 }
