@@ -29,9 +29,12 @@ class CameraParams(ctypes.Structure):
     ]
 
 
-def make_cameras(R, c, f, k, constrained=None, constraints=None, weights=None, known=None, K_known=None, k_known=None):
+def make_cameras(R, c, f, k, constrained=None, constraints=None, weights=None, known=None, K_known=None, k_known=None,
+                 fisheye=None, fisheye_params=None):
     """camera_params_t array.  known (m flags), K_known (m x 9) and k_known (m x 5) describe calibrated cameras
-    (known_intrinsics, lib/sfm-driver/sfm.c:339-357); without them every camera is an ordinary one."""
+    (known_intrinsics, lib/sfm-driver/sfm.c:339-357); without them every camera is an ordinary one.  fisheye (m flags)
+    and fisheye_params (m x 5: f_cx, f_cy, f_rad, f_angle, f_focal) fill the fisheye fields (src/Bundle.cpp:234-239),
+    which only the fisheye projection reads (optimize_for_fisheye)."""
     m = len(f)
     cams = (CameraParams * m)()
     for j in range(m):
@@ -50,6 +53,10 @@ def make_cameras(R, c, f, k, constrained=None, constraints=None, weights=None, k
             cams[j].known_intrinsics = b"\x01"
             cams[j].K_known[:] = list(np.asarray(K_known[j], float).reshape(9))
             cams[j].k_known[:] = list(np.asarray(k_known[j], float).reshape(5))
+        if fisheye is not None and fisheye[j]:
+            cams[j].fisheye = b"\x01"
+        if fisheye_params is not None:
+            (cams[j].f_cx, cams[j].f_cy, cams[j].f_rad, cams[j].f_angle, cams[j].f_focal) = (float(v) for v in fisheye_params[j])
     return cams
 
 
@@ -104,13 +111,16 @@ def observations(scene):
 def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_centers=1, ncons=0, eps2=1e-12,
                  use_constraints=0, constrained=None, constraints=None, weights=None,
                  use_point_constraints=0, points_constraints=None, point_constraint_weight=0.0,
-                 extra_info=False, export=False, fix_points=0, known=None, K_known=None, k_known=None):
+                 extra_info=False, export=False, fix_points=0, known=None, K_known=None, k_known=None,
+                 fisheye=None, fisheye_params=None, optimize_for_fisheye=0):
     """Calls a run_sfm-shaped C function (ours or the reference's) on a scene dict (synth.ba_scene), or
-    bsfm_run_sfm_crs on a CRS scene (synth.crs_scene).  known / K_known / k_known: calibrated cameras (see make_cameras).
+    bsfm_run_sfm_crs on a CRS scene (synth.crs_scene).  known / K_known / k_known: calibrated cameras, fisheye /
+    fisheye_params: fisheye cameras (see make_cameras); optimize_for_fisheye is passed to the callee.
     Returns a dict with the refined R, c, f, k, pts (+ info when the callee provides it)."""
     n, m, vis_args, _keep = _visibility_args(scene)
     proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
-    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], constrained, constraints, weights, known, K_known, k_known)
+    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], constrained, constraints, weights, known, K_known, k_known,
+                        fisheye, fisheye_params)
     pts = np.ascontiguousarray(scene["pts"], dtype=np.float64).copy()
     pc = None
     if use_point_constraints:
@@ -122,7 +132,8 @@ def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_cen
         ex = {"V": np.zeros((n, 9)), "S": np.zeros((m * cnp, m * cnp)), "U": np.zeros((m, cnp * cnp)), "W": np.zeros((m * cnp, 3 * n))}
     args = [n, m, ncons, *vis_args, proj.ctypes.data, est_focal_length, 0, undistort, explicit_camera_centers,
             ctypes.addressof(cams), pts.ctypes.data, use_constraints, use_point_constraints,
-            pc.ctypes.data if pc is not None else None, float(point_constraint_weight), int(fix_points), 0, float(eps2),
+            pc.ctypes.data if pc is not None else None, float(point_constraint_weight), int(fix_points), int(optimize_for_fisheye),
+            float(eps2),
             ex["V"].ctypes.data if export and "V" in export_keys else None, ex["S"].ctypes.data if export and "S" in export_keys else None,
             ex["U"].ctypes.data if export and "U" in export_keys else None, ex["W"].ctypes.data if export and "W" in export_keys else None]
     info = np.zeros(10)
@@ -137,15 +148,19 @@ def call_run_sfm(fn, scene, est_focal_length=1, undistort=1, explicit_camera_cen
 _run_sfm = {}
 
 
-def run_sfm(scene, **kw):
+def run_sfm(scene, optimize_for_fisheye=None, **kw):
     """GPU run_sfm: bsfm_run_sfm, or bsfm_run_sfm_crs for a scene with vis_ptr / vis_cam instead of vmask.  Raises on BSFM
     errors; returns the refined scene + info[10].  Keywords are those of call_run_sfm (known / K_known / k_known for
-    calibrated cameras)."""
+    calibrated cameras, fisheye / fisheye_params for fisheye cameras).  With optimize_for_fisheye set (0 or 1) the call
+    goes to bsfm_run_sfm_fe / bsfm_run_sfm_crs_fe with that value."""
     name = "bsfm_run_sfm_crs" if "vis_ptr" in scene else "bsfm_run_sfm"
+    if optimize_for_fisheye is not None:
+        name += "_fe"
+        kw["optimize_for_fisheye"] = optimize_for_fisheye
     if name not in _run_sfm:
         fn = getattr(load_library(), name)
         _bind_run_sfm(fn)
-        if name.endswith("_crs"):   # vmask -> vis_ptr, vis_cam, nvis
+        if "_crs" in name:   # vmask -> vis_ptr, vis_cam, nvis
             fn.argtypes = fn.argtypes[:3] + [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + fn.argtypes[4:]
         fn.argtypes = fn.argtypes + [ctypes.c_void_p]
         fn.restype = ctypes.c_int
@@ -261,17 +276,22 @@ def unpack_params(p, scene, est_focal_length=1, undistort=1, f_scale=0.001, k_sc
 
 
 def levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, cnp, R_init, f_fixed, est_focal_length=1, undistort=1,
-                 explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, eps5=4.0e-2, init_params=None):
+                 explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, eps5=4.0e-2, init_params=None,
+                 optimize_for_fisheye=None):
     """bsfm_sba_motstr_levmar_model with raw (host or DEVICE) pointers for vmask / p / x.
     init_params: a make_cameras array whose calibrated cameras the projection uses (bsfm_sba_motstr_levmar_model_ki).
+    optimize_for_fisheye (0 or 1, with init_params): bsfm_sba_motstr_levmar_model_fe, the fisheye projection with 1.
     Returns (iterations, info[10])."""
     lib = load_library()
     name = "bsfm_sba_motstr_levmar_model" if init_params is None else "bsfm_sba_motstr_levmar_model_ki"
+    if optimize_for_fisheye is not None:
+        name = "bsfm_sba_motstr_levmar_model_fe"
     fn = getattr(lib, name)
     c = ctypes
     fn.argtypes = [c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int,
                    c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p, c.c_int, c.c_void_p,
-                   c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p] + ([] if init_params is None else [c.c_void_p])
+                   c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p] + ([] if init_params is None and optimize_for_fisheye is None else [c.c_void_p]) + \
+        ([] if optimize_for_fisheye is None else [c.c_int])
     fn.restype = c.c_int
     R_init = np.ascontiguousarray(R_init, dtype=np.float64)
     f_fixed = np.ascontiguousarray(f_fixed, dtype=np.float64)
@@ -280,7 +300,9 @@ def levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, cnp, R_init, f_fixed, est_focal_
     info = np.zeros(10)
     args = [n, m, 0, vmask_ptr, p_ptr, cnp, 3, x_ptr, None, 2, ctypes.addressof(model), jac_mode, itmax, verbose,
             opts.ctypes.data, info.ctypes.data, 0, None, 0, None, None, None, None, None]
-    if init_params is not None:
+    if optimize_for_fisheye is not None:
+        args += [None if init_params is None else ctypes.addressof(init_params), int(optimize_for_fisheye)]
+    elif init_params is not None:
         args.append(ctypes.addressof(init_params))
     rc = fn(*args)
     if rc < -1:
@@ -289,16 +311,19 @@ def levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, cnp, R_init, f_fixed, est_focal_
 
 
 def mot_levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, points_ptr, cnp, R_init, f_fixed, est_focal_length=1, undistort=1,
-                     explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, init_params=None):
-    """motion-only counterpart of levmar_model: bsfm_sba_mot_levmar_model(_ki) with raw (host or DEVICE) pointers for
+                     explicit_camera_centers=1, eps2=1e-12, itmax=150, verbose=0, jac_mode=0, init_params=None,
+                     optimize_for_fisheye=None):
+    """motion-only counterpart of levmar_model: bsfm_sba_mot_levmar_model(_ki / _fe) with raw (host or DEVICE) pointers for
     vmask / p (cameras only) / x / points (n x 3, fixed).  Returns (iterations, info[10])."""
     lib = load_library()
     name = "bsfm_sba_mot_levmar_model" if init_params is None else "bsfm_sba_mot_levmar_model_ki"
+    if optimize_for_fisheye is not None:
+        name = "bsfm_sba_mot_levmar_model_fe"
     fn = getattr(lib, name)
     c = ctypes
     fn.argtypes = [c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p, c.c_void_p, c.c_int,
                    c.c_void_p, c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p] + \
-        ([] if init_params is None else [c.c_void_p])
+        ([] if init_params is None and optimize_for_fisheye is None else [c.c_void_p]) + ([] if optimize_for_fisheye is None else [c.c_int])
     fn.restype = c.c_int
     R_init = np.ascontiguousarray(R_init, dtype=np.float64)
     f_fixed = np.ascontiguousarray(f_fixed, dtype=np.float64)
@@ -307,7 +332,9 @@ def mot_levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, points_ptr, cnp, R_init, f_f
     info = np.zeros(10)
     args = [n, m, 0, vmask_ptr, p_ptr, cnp, x_ptr, None, 2, ctypes.addressof(model), points_ptr, jac_mode, itmax, verbose,
             opts.ctypes.data, info.ctypes.data, 0, None]
-    if init_params is not None:
+    if optimize_for_fisheye is not None:
+        args += [None if init_params is None else ctypes.addressof(init_params), int(optimize_for_fisheye)]
+    elif init_params is not None:
         args.append(ctypes.addressof(init_params))
     rc = fn(*args)
     if rc < -1:
@@ -316,24 +343,27 @@ def mot_levmar_model(n, m, vmask_ptr, p_ptr, x_ptr, points_ptr, cnp, R_init, f_f
 
 
 def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thresh=16.0, pt_protected=None, cap=None,
-                          known=None, K_known=None, k_known=None):
+                          known=None, K_known=None, k_known=None, fisheye=None, fisheye_params=None, optimize_for_fisheye=None):
     """bsfm_reprojection_outliers: the statistics / outlier pass BundlerApp::RunSFM_SBA runs after every run_sfm
     (src/Bundle.cpp:659-856) on a scene dict (vmask, projections, R, c, f, k, pts), or bsfm_reprojection_outliers_crs on a
     CRS scene (vis_ptr / vis_cam instead of vmask, see synth.crs_scene).  Defaults are bundler's
     m_min/max_proj_error_threshold (BundlerApp.h).  Returns dist[nvis], stats[m x 5] (n, mean, median, med80, thresh),
-    outliers, errors, global_mean.  known / K_known / k_known: calibrated cameras, as for run_sfm."""
+    outliers, errors, global_mean.  known / K_known / k_known: calibrated cameras, fisheye / fisheye_params: fisheye
+    cameras, as for run_sfm.  With optimize_for_fisheye set (0 or 1) the call goes to the _fe entry with that value."""
     lib = load_library()
     crs = "vis_ptr" in scene
-    name = "bsfm_reprojection_outliers_crs" if crs else "bsfm_reprojection_outliers"
+    fe = optimize_for_fisheye is not None
+    name = ("bsfm_reprojection_outliers_crs" if crs else "bsfm_reprojection_outliers") + ("_fe" if fe else "")
     fn = getattr(lib, name)
     fn.restype = ctypes.c_int
     vis_types = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] if crs else [ctypes.c_void_p]
-    fn.argtypes = [ctypes.c_int, ctypes.c_int] + vis_types + [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
-                   ctypes.c_double, ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+    fn.argtypes = [ctypes.c_int, ctypes.c_int] + vis_types + [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + \
+        ([ctypes.c_int] if fe else []) + [ctypes.c_double, ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                    ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
     n, m, vis_args, _keep = _visibility_args(scene)
     proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
-    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], known=known, K_known=K_known, k_known=k_known)
+    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], known=known, K_known=K_known, k_known=k_known,
+                        fisheye=fisheye, fisheye_params=fisheye_params)
     pts = np.ascontiguousarray(scene["pts"], dtype=np.float64)
     prot = None if pt_protected is None else np.ascontiguousarray(pt_protected, dtype=np.int8)
     nvis = proj.shape[0]
@@ -342,7 +372,7 @@ def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thre
     out_idx = np.zeros(max(cap, 1), np.int32); out_err = np.zeros(max(cap, 1))
     gm = ctypes.c_double()
     rc = fn(n, m, *vis_args, proj.ctypes.data, ctypes.addressof(cams), pts.ctypes.data, int(estimate_distortion),
-            float(min_thresh), float(max_thresh), None if prot is None else prot.ctypes.data, stats.ctypes.data, dist.ctypes.data,
+            *([int(optimize_for_fisheye)] if fe else []), float(min_thresh), float(max_thresh), None if prot is None else prot.ctypes.data, stats.ctypes.data, dist.ctypes.data,
             out_idx.ctypes.data, out_err.ctypes.data, cap, ctypes.byref(gm))
     check(rc, name)
     k = min(rc, cap)

@@ -6,6 +6,8 @@
 //                    sfm_project_point3     lib/sfm-driver/sfm.c:503-552
 //                    sfm_project_rd         lib/sfm-driver/sfm.c:302-380
 //                    rot_update             lib/sfm-driver/sfm.c:77-116
+//                    sfm_project_point2_fisheye  lib/sfm-driver/sfm.c:448-492 (FE kernels; sfm_project2 :243-299,
+//                                           sfm_fisheye_distort :426-446)
 //   K2 Jacobian      sba_motstr_Qs_fdjac    lib/sba-1.5/sba_levmar_wrap.c:163-259  (FD mode)
 //                    snavely_reprojection_error.h:58-92 / SURVEY.md A.4            (analytic mode)
 //   K3 U,ea / V,eb / W                      lib/sba-1.5/sba_levmar.c:919-964 / 987-1030 / 1053-1082
@@ -123,9 +125,12 @@ __device__ __forceinline__ double fd_step(double v)
 // sfm_project_point3 + sfm_project_rd (lib/sfm-driver/sfm.c:503-552, 302-380).  KI = false: every camera takes the
 // known_intrinsics = 0 branch and `ci` is not read.  KI = true: calibrated cameras (ci->known) take the other branch;
 // the radial step after it is the same for both and still uses the focal parameter K0.
-template <bool KI>
-__device__ __forceinline__ void project_dev(const Model &M, const CamIntrinsics *ci, const double (&a)[MAX_CNP], const double *R,
-                                            double f_fixed, double b0, double b1, double b2, double &px, double &py)
+// FE = true: sfm_project_point2_fisheye (sfm.c:448-492) instead: the same pinhole (sfm_project2, :243-299) without the
+// radial step, then the fisheye mapping for cameras with cf->fisheye (sfm_fisheye_distort, :426-446).  FE = false never
+// reads `cf`.
+template <bool KI, bool FE>
+__device__ __forceinline__ void project_dev(const Model &M, const CamIntrinsics *ci, const CamFisheye *cf, const double (&a)[MAX_CNP],
+                                            const double *R, double f_fixed, double b0, double b1, double b2, double &px, double &py)
 {
     double bc0, bc1, bc2;
     if (M.explicit_centers) {
@@ -147,7 +152,9 @@ __device__ __forceinline__ void project_dev(const Model &M, const CamIntrinsics 
         p0 = -bc0 * K0 / bc2;
         p1 = -bc1 * K0 / bc2;
     }
-    if (M.undistort) {
+    if (FE) {
+        if (cf->fisheye) fisheye_distort_dev(*cf, p0, p1, p0, p1);
+    } else if (M.undistort) {
         const double k1 = (M.est_focal ? a[7] : a[6]) / M.k_scale;
         const double k2 = (M.est_focal ? a[8] : a[7]) / M.k_scale;
         const double rsq = (p0 * p0 + p1 * p1) / (K0 * K0);
@@ -194,7 +201,7 @@ __global__ void cam_prep_kernel(Problem P, const double *p, int with_pert)
 // K1: e = x - f(p), sum e^2 (sba_levmar.c:802-806, nrmL2xmy :159-207)
 // also: stop-8 statistic against a previous residual vector when e_prev != nullptr (:1552-1561)
 // ------------------------------------------------------------------------------------------------
-template <bool KI>
+template <bool KI, bool FE>
 __global__ void residual_kernel(Problem P, const double *p, double *e_out, const double *e_prev, double eps5)
 {
     cudaGridDependencySynchronize();   // programmatic dependent launch (see launch_pdl)
@@ -206,7 +213,8 @@ __global__ void residual_kernel(Problem P, const double *p, double *e_out, const
         load_cam(P, p, j, a);
         const double *b = p + (size_t) P.m * P.M.cnp + (size_t) i * 3;
         double hx, hy;
-        project_dev<KI>(P.M, KI ? P.intr + j : nullptr, a, P.camR + (size_t) j * 36, P.f_fixed[j], b[0], b[1], b[2], hx, hy);
+        project_dev<KI, FE>(P.M, KI ? P.intr + j : nullptr, FE ? P.fe + j : nullptr, a, P.camR + (size_t) j * 36, P.f_fixed[j],
+                            b[0], b[1], b[2], hx, hy);
         const double e0 = P.x[2 * (size_t) o] - hx, e1 = P.x[2 * (size_t) o + 1] - hy;
         e_out[2 * (size_t) o] = e0;
         e_out[2 * (size_t) o + 1] = e1;
@@ -227,15 +235,18 @@ __global__ void residual_kernel(Problem P, const double *p, double *e_out, const
         if (grid_reduce<1>(pct, P.partial + gridDim.x, P.ticket + 1, out)) P.sc->max_pct = out;
     }
 }
-template __global__ void residual_kernel<false>(Problem, const double *, double *, const double *, double);
-template __global__ void residual_kernel<true>(Problem, const double *, double *, const double *, double);
+template __global__ void residual_kernel<false, false>(Problem, const double *, double *, const double *, double);
+template __global__ void residual_kernel<true, false>(Problem, const double *, double *, const double *, double);
+template __global__ void residual_kernel<false, true>(Problem, const double *, double *, const double *, double);
+template __global__ void residual_kernel<true, true>(Problem, const double *, double *, const double *, double);
 
 // ------------------------------------------------------------------------------------------------
 // K2 + W of K3: per observation A_ij (2 x cnp), B_ij (2 x 3), W_ij = A^T B (cnp x 3)
 // ------------------------------------------------------------------------------------------------
-template <bool KI>
-__device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsics *ci, const double (&a)[MAX_CNP], const double *R0,
-                                             double f_fixed, double b0, double b1, double b2, double (&A)[2][MAX_CNP], double (&B)[2][3])
+template <bool KI, bool FE>
+__device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsics *ci, const CamFisheye *cf, const double (&a)[MAX_CNP],
+                                             const double *R0, double f_fixed, double b0, double b1, double b2, double (&A)[2][MAX_CNP],
+                                             double (&B)[2][3])
 {
     // SURVEY.md A.4.  v = R_init (X - c) [or R_init X], Pc = exp([w]x) v (+ t), q = -Pc.xy / Pc.z
     const Model &M = P.M;
@@ -250,14 +261,17 @@ __device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsi
     // rotated part (without translation) is what d/dw acts on
     const double Pr0 = Pc0, Pr1 = Pc1, Pr2 = Pc2;
     if (!M.explicit_centers) { Pc0 += a[0]; Pc1 += a[1]; Pc2 += a[2]; }
+    // the fisheye projection has no radial step: its k columns are zero
+    const bool radial = M.undistort && !FE;
     const double f = M.est_focal ? a[6] / M.f_scale : f_fixed;
-    const double k1 = M.undistort ? (M.est_focal ? a[7] : a[6]) / M.k_scale : 0.0;
-    const double k2 = M.undistort ? (M.est_focal ? a[8] : a[7]) / M.k_scale : 0.0;
+    const double k1 = radial ? (M.est_focal ? a[7] : a[6]) / M.k_scale : 0.0;
+    const double k2 = radial ? (M.est_focal ? a[8] : a[7]) / M.k_scale : 0.0;
     const double iz = 1.0 / Pc2;
     const double q0 = -Pc0 * iz, q1 = -Pc1 * iz;
     double G[2][3];
     double Ai[2][3];   // calibrated camera: columns of f*f_scale, k1*k_scale, k2*k_scale (sfm.c:673-681)
     double rho, r;
+    double ph0, ph1;   // the pinhole projection, what the fisheye mapping acts on
     if (KI && ci->known) {
         // calibrated camera: u = Kc d(q) (Brown-Conrady d, Kc = [[K0, K1], [0, K4]]), then the radial step
         // xhat = u (1 + k1 s + k2 s^2), s = |u|^2 / f^2.  dxhat/dq = (fac I + h u u^T) Kc Jd, h = 2 (k1 + 2 k2 s) / f^2
@@ -274,17 +288,18 @@ __device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsi
         const double M00 = Kc[0] * J00 + Kc[1] * J01, M01 = Kc[0] * J01 + Kc[1] * J11;
         const double M10 = Kc[3] * J01, M11 = Kc[3] * J11;
         const double u0 = Kc[0] * xd + Kc[1] * yd + Kc[2], u1 = Kc[3] * yd + Kc[4];
+        ph0 = u0; ph1 = u1;
         // without the radial step f is not read at all (it may be unset when it is not estimated either)
-        const double s = M.undistort ? (u0 * u0 + u1 * u1) / (f * f) : 0.0;
+        const double s = radial ? (u0 * u0 + u1 * u1) / (f * f) : 0.0;
         const double fac = 1.0 + k1 * s + k2 * s * s;
-        const double h = M.undistort ? 2.0 * (k1 + 2.0 * k2 * s) / (f * f) : 0.0;
+        const double h = radial ? 2.0 * (k1 + 2.0 * k2 * s) / (f * f) : 0.0;
         const double P00 = fac + h * u0 * u0, P01 = h * u0 * u1, P11 = fac + h * u1 * u1;
         const double D00 = P00 * M00 + P01 * M10, D01 = P00 * M01 + P01 * M11;
         const double D10 = P01 * M00 + P11 * M10, D11 = P01 * M01 + P11 * M11;
         G[0][0] = -iz * D00; G[0][1] = -iz * D01; G[0][2] = -iz * (D00 * q0 + D01 * q1);
         G[1][0] = -iz * D10; G[1][1] = -iz * D11; G[1][2] = -iz * (D10 * q0 + D11 * q1);
         // the focal length enters only through s (zero column without the radial step)
-        const double dsf = M.undistort ? -2.0 * s / f * (k1 + 2.0 * k2 * s) : 0.0;
+        const double dsf = radial ? -2.0 * s / f * (k1 + 2.0 * k2 * s) : 0.0;
         const double uu[2] = {u0, u1};
 #pragma unroll
         for (int k = 0; k < 2; k++) {
@@ -302,6 +317,25 @@ __device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsi
         // G = dxhat/dPc (2x3)
         G[0][0] = -iz * D00; G[0][1] = -iz * D01; G[0][2] = -iz * (D00 * q0 + D01 * q1);
         G[1][0] = -iz * D01; G[1][1] = -iz * D11; G[1][2] = -iz * (D01 * q0 + D11 * q1);
+        ph0 = f * q0; ph1 = f * q1;
+    }
+    // fisheye mapping x_d = g(|u|) u + c of the pinhole output u, g(r) = s atan(r / F) / r, s = (180 / pi) f_rad / (f_angle / 2):
+    // dx_d/du = g I + (g'(r) / r) u u^T, g'(r) / r = (s / (F (1 + (r / F)^2)) - g) / r^2
+    double Jf00 = 1.0, Jf01 = 0.0, Jf11 = 1.0;
+    const bool fish = FE && cf->fisheye;
+    if (fish) {
+        const double rr = ph0 * ph0 + ph1 * ph1, rf = sqrt(rr);
+        const double sc = (180.0 / BSFM_M_PI) * cf->rad / (0.5 * cf->angle);
+        const double x = rf / cf->focal;
+        const double g = sc * atan(x) / rf;
+        const double gp = (sc / (cf->focal * (1.0 + x * x)) - g) / rr;
+        Jf00 = g + gp * ph0 * ph0; Jf01 = gp * ph0 * ph1; Jf11 = g + gp * ph1 * ph1;
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            const double g0 = G[0][c], g1 = G[1][c];
+            G[0][c] = Jf00 * g0 + Jf01 * g1;
+            G[1][c] = Jf01 * g0 + Jf11 * g1;
+        }
     }
     // B = G R ; dPc/dc = -R (explicit centres) or dPc/dt = I
 #pragma unroll
@@ -338,19 +372,27 @@ __device__ __forceinline__ void analytic_jac(const Problem &P, const CamIntrinsi
         for (int c = 0; c < 3; c++) A[k][3 + c] = G[k][0] * dPdw[c] + G[k][1] * dPdw[3 + c] + G[k][2] * dPdw[6 + c];
     // intrinsics
     const double qq[2] = {q0, q1};
+    double dfs_v[2];
+#pragma unroll
+    for (int k = 0; k < 2; k++) dfs_v[k] = (KI && ci->known) ? Ai[k][0] : r * qq[k] / M.f_scale;
+    if (fish) {
+        const double d0 = dfs_v[0], d1 = dfs_v[1];
+        dfs_v[0] = Jf00 * d0 + Jf01 * d1;
+        dfs_v[1] = Jf01 * d0 + Jf11 * d1;
+    }
 #pragma unroll
     for (int k = 0; k < 2; k++) {
         const bool kn = KI && ci->known;
-        const double dfs = kn ? Ai[k][0] : r * qq[k] / M.f_scale;
-        const double dk1 = kn ? Ai[k][1] : f * rho * qq[k] / M.k_scale;
-        const double dk2 = kn ? Ai[k][2] : f * rho * rho * qq[k] / M.k_scale;
+        const double dfs = dfs_v[k];
+        const double dk1 = FE ? 0.0 : (kn ? Ai[k][1] : f * rho * qq[k] / M.k_scale);
+        const double dk2 = FE ? 0.0 : (kn ? Ai[k][2] : f * rho * rho * qq[k] / M.k_scale);
         A[k][6] = M.est_focal ? dfs : (M.undistort ? dk1 : 0.0);
         A[k][7] = M.est_focal ? (M.undistort ? dk1 : 0.0) : (M.undistort ? dk2 : 0.0);
         A[k][8] = (M.est_focal && M.undistort) ? dk2 : 0.0;
     }
 }
 
-template <bool KI>
+template <bool KI, bool FE>
 __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *p, int jac_mode)
 {
     cudaGridDependencySynchronize();   // programmatic dependent launch (see launch_pdl)
@@ -365,14 +407,15 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
     double b[3] = {bp[0], bp[1], bp[2]};
     const double ff = P.f_fixed[j];
     const CamIntrinsics *ci = KI ? P.intr + j : nullptr;
+    const CamFisheye *cf = FE ? P.fe + j : nullptr;
     double A[2][MAX_CNP], B[2][3];
 
     if (jac_mode == 1) {
-        analytic_jac<KI>(P, ci, a, P.R_init + (size_t) j * 9, ff, b[0], b[1], b[2], A, B);
+        analytic_jac<KI, FE>(P, ci, cf, a, P.R_init + (size_t) j * 9, ff, b[0], b[1], b[2], A, B);
     } else {
         const double *Rb = P.camR + (size_t) j * 36;
         double h0, h1;
-        project_dev<KI>(M, ci, a, Rb, ff, b[0], b[1], b[2], h0, h1);
+        project_dev<KI, FE>(M, ci, cf, a, Rb, ff, b[0], b[1], b[2], h0, h1);
 #pragma unroll
         for (int jj = 0; jj < MAX_CNP; jj++) {
             A[0][jj] = 0.0; A[1][jj] = 0.0;
@@ -383,7 +426,7 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
                 a[jj] = tmp + d;
                 const double *R = (jj >= 3 && jj <= 5) ? (Rb + 9 * (jj - 2)) : Rb;
                 double g0, g1;
-                project_dev<KI>(M, ci, a, R, ff, b[0], b[1], b[2], g0, g1);
+                project_dev<KI, FE>(M, ci, cf, a, R, ff, b[0], b[1], b[2], g0, g1);
                 a[jj] = tmp;
                 A[0][jj] = (g0 - h0) * d1;
                 A[1][jj] = (g1 - h1) * d1;
@@ -396,7 +439,7 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
             const double tmp = b[jj];
             b[jj] = tmp + d;
             double g0, g1;
-            project_dev<KI>(M, ci, a, Rb, ff, b[0], b[1], b[2], g0, g1);
+            project_dev<KI, FE>(M, ci, cf, a, Rb, ff, b[0], b[1], b[2], g0, g1);
             b[jj] = tmp;
             B[0][jj] = (g0 - h0) * d1;
             B[1][jj] = (g1 - h1) * d1;
@@ -423,8 +466,10 @@ __global__ void __launch_bounds__(128) jacobian_kernel(Problem P, const double *
 #pragma unroll
     for (int jj = 0; jj < 3; jj++) { jB[jj] = B[0][jj]; jB[3 + jj] = B[1][jj]; }
 }
-template __global__ void jacobian_kernel<false>(Problem, const double *, int);
-template __global__ void jacobian_kernel<true>(Problem, const double *, int);
+template __global__ void jacobian_kernel<false, false>(Problem, const double *, int);
+template __global__ void jacobian_kernel<true, false>(Problem, const double *, int);
+template __global__ void jacobian_kernel<false, true>(Problem, const double *, int);
+template __global__ void jacobian_kernel<true, true>(Problem, const double *, int);
 
 // ------------------------------------------------------------------------------------------------
 // K3: V_i, eb_i -- one thread per point, observations in ascending camera order (same summation

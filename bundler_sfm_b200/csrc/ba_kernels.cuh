@@ -63,6 +63,36 @@ __device__ __forceinline__ void project_known_dev(const CamIntrinsics &ci, doubl
     p1 = ci.K[3] * y_d + ci.K[4];
 }
 
+// Fisheye camera (camera_params_t::fisheye, f_cx, f_cy, f_rad, f_angle, f_focal; lib/sfm-driver/sfm.c:426-446): the
+// equidistant mapping applied after the pinhole.  Uploaded once per solve, and only when the call asks for the fisheye
+// projection (optimize_for_fisheye).
+struct CamFisheye {
+    double cx, cy, rad, angle, focal;
+    int fisheye;    // fisheye != 0
+    int pad;
+};
+
+inline CamFisheye cam_fisheye(const bsfm_camera_params_t &c)
+{
+    CamFisheye cf;
+    cf.cx = c.f_cx; cf.cy = c.f_cy; cf.rad = c.f_rad; cf.angle = c.f_angle; cf.focal = c.f_focal;
+    cf.fisheye = c.fisheye ? 1 : 0;
+    cf.pad = 0;
+    return cf;
+}
+
+constexpr double BSFM_M_PI = 3.14159265358979323846;   // M_PI of the reference's libc headers
+
+// r -> rnew of sfm_fisheye_distort (sfm.c:439-445) in the reference's operation order; r = 0 gives NaN, as there
+__device__ __forceinline__ void fisheye_distort_dev(const CamFisheye &cf, double x, double y, double &xd, double &yd)
+{
+    const double r = sqrt(x * x + y * y);
+    const double angle = 180.0 * atan(r / cf.focal) / BSFM_M_PI;
+    const double rnew = cf.rad * angle / (0.5 * cf.angle);
+    xd = x * (rnew / r) + cf.cx;
+    yd = y * (rnew / r) + cf.cy;
+}
+
 // scalars produced on the device, copied to pinned host memory once per LM phase
 struct Scalars {
     double e_L2;          // sum e^2 of the last residual evaluation
@@ -126,6 +156,7 @@ struct Problem {
     Scalars *sc;      // device scalars
     const double *mu; // damping term of the current try (device scalar, written by the host)
     const CamIntrinsics *intr;  // m entries, or null when no camera is calibrated (then only the KI = false kernels run)
+    const CamFisheye *fe;       // m entries, or null without the fisheye projection (then only the FE = false kernels run)
 };
 
 // launch with the programmatic-stream-serialization attribute (PDL): the launch latency of a kernel overlaps
@@ -145,8 +176,8 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, c
 
 // kernels of ba_kernels.cu that the LM solver (ba_solver.cu) launches
 __global__ void cam_prep_kernel(Problem P, const double *p, int with_pert);
-template <bool KI> __global__ void residual_kernel(Problem P, const double *p, double *e_out, const double *e_prev, double eps5);
-template <bool KI> __global__ void jacobian_kernel(Problem P, const double *p, int jac_mode);
+template <bool KI, bool FE> __global__ void residual_kernel(Problem P, const double *p, double *e_out, const double *e_prev, double eps5);
+template <bool KI, bool FE> __global__ void jacobian_kernel(Problem P, const double *p, int jac_mode);
 __global__ void v_kernel(Problem P, const double *p, const double *e);
 __global__ void u_partial_kernel(Problem P, const double *e, int nseg);
 __global__ void u_final_kernel(Problem P, const double *p, int nseg);

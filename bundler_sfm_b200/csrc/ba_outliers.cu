@@ -1,6 +1,8 @@
 // ba_outliers.cu -- the reprojection statistics / outlier pass that BundlerApp::RunSFM_SBA runs after every
 // run_sfm (src/Bundle.cpp:659-856), on the arguments run_sfm just used (SURVEY.md 8f row 1).
 //   per observation : dist = || sfm_project_rd(camera, point) - key ||            (Bundle.cpp:721-754, sfm.c:302-380)
+//                     with optimize_for_fisheye, ImageData::DistortPoint after the projection (Bundle.cpp:746-751,
+//                     ImageData.cpp:1129-1169)
 //   per camera      : med = kth_element_copy(n, iround(0.8 n), dists)             (Bundle.cpp:761-764; qsort.c:152-204:
 //                     the k-th smallest, 0.0 when k >= n), thresh = CLAMP(1.2 * 2.0 * med, min, max) (:768-771),
 //                     mean and median (iround(0.5 n)) for the log line (:776-788)
@@ -24,12 +26,34 @@ namespace bsfm {
 namespace ba {
 
 struct CamCompact { double R[9], t[3], f, k0, k1; };
+struct Rot3 { double R[9]; };
+
+// ImageData::DistortPoint (ImageData.cpp:1129-1169) of a fisheye camera, in the reference's operation order: the ray
+// (x, y, -f_focal) is rotated by `Rs`; when its z is not positive the point is left as it is (the reference returns
+// without writing its aliased output), else it is re-projected and mapped like sfm_fisheye_distort, with
+// RAD2DEG(a) = a * (180 / pi) (imagelib/defines.h:32)
+__device__ __forceinline__ void distort_point_dev(const CamFisheye &cf, const Rot3 &Rs, double &x, double &y)
+{
+    const double F = cf.focal;
+    const double r0 = Rs.R[0] * x + Rs.R[1] * y + Rs.R[2] * -F;
+    const double r1 = Rs.R[3] * x + Rs.R[4] * y + Rs.R[5] * -F;
+    const double r2 = Rs.R[6] * x + Rs.R[7] * y + Rs.R[8] * -F;
+    if (r2 <= 0.0) return;
+    const double xn = r0 * F / r2;
+    const double yn = r1 * F / r2;
+    const double r = sqrt(xn * xn + yn * yn);
+    const double angle = atan(r / F) * (180.0 / BSFM_M_PI);
+    const double rnew = cf.rad * angle / (0.5 * cf.angle);
+    x = xn * (rnew / r) + cf.cx;
+    y = yn * (rnew / r) + cf.cy;
+}
 
 // one thread per observation (point-major order == the order of `projections`).  KI: `intr` (m entries) holds the
-// calibrated cameras; KI = false never reads it.
-template <bool KI>
+// calibrated cameras; KI = false never reads it.  FE: `fe` (m entries) holds the fisheye cameras, whose projections
+// DistortPoint maps with `Rs`; FE = false never reads them.
+template <bool KI, bool FE>
 __global__ void outlier_dist_kernel(int nvis, const int *obs_cam, const int *obs_pt, const CamCompact *cams, const CamIntrinsics *intr,
-                                    const double *pts, const double *proj, int undistort, double *dist)
+                                    const CamFisheye *fe, Rot3 Rs, const double *pts, const double *proj, int undistort, double *dist)
 {
     const int o = blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= nvis) return;
@@ -53,6 +77,7 @@ __global__ void outlier_dist_kernel(int nvis, const int *obs_cam, const int *obs
         p0 *= factor;
         p1 *= factor;
     }
+    if (FE && fe[obs_cam[o]].fisheye) distort_point_dev(fe[obs_cam[o]], Rs, p0, p1);
     const double dx = p0 - proj[2 * (size_t) o], dy = p1 - proj[2 * (size_t) o + 1];
     dist[o] = sqrt(dx * dx + dy * dy);     // Bundle.cpp:753-756
 }
@@ -112,8 +137,8 @@ using namespace bsfm::ba;
 
 // the outlier pass on either visibility source (bsfm_reprojection_outliers, bsfm_reprojection_outliers_crs)
 static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src, const double *projections,
-                         const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion,
-                         double min_proj_error_threshold, double max_proj_error_threshold,
+                         const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion, int fisheye_entry,
+                         int optimize_for_fisheye, double min_proj_error_threshold, double max_proj_error_threshold,
                          const char *pt_protected, double *cam_stats, double *obs_dist,
                          int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
 {
@@ -126,7 +151,7 @@ static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src,
     }
     bool any_known = false;
     for (int j = 0; j < m; j++) {
-        if (cams[j].fisheye) { set_error("bsfm_reprojection_outliers: fisheye cameras are outside the GPU path"); return BSFM_ERR_UNSUPPORTED; }
+        if (cams[j].fisheye && !fisheye_entry) { set_error("bsfm_reprojection_outliers: fisheye cameras are outside this entry; bsfm_reprojection_outliers_fe takes them"); return BSFM_ERR_UNSUPPORTED; }
         any_known = any_known || cams[j].known_intrinsics;
     }
 
@@ -157,12 +182,33 @@ static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src,
         for (int j = 0; j < m; j++) hi[j] = cam_intrinsics(cams[j]);
         TRY(D.upload(&d_intr, hi.data(), (size_t) m));
     }
+    CamFisheye *d_fe = nullptr;         // fisheye cameras: side table, only when the call asks for their mapping
+    Rot3 Rs = {};
+    if (optimize_for_fisheye) {
+        std::vector<CamFisheye> hf(m);
+        for (int j = 0; j < m; j++) hf[j] = cam_fisheye(cams[j]);
+        TRY(D.upload(&d_fe, hf.data(), (size_t) m));
+        // GetRotationFromSpherical(-pi/2, pi/2) (BundleUtil.cpp:70-94), with the host libm like the reference: the identity
+        // up to +-6.1e-17 terms, which change the last bits of the result
+        const double theta = -0.5 * M_PI, phi = 0.5 * M_PI;
+        const double v[3] = {cos(theta) * sin(phi), cos(phi), sin(theta) * sin(phi)};
+        const double phi_up = phi - 0.5 * M_PI, theta_up = theta;
+        const double up[3] = {cos(theta_up) * sin(phi_up), cos(phi_up), sin(theta_up) * sin(phi_up)};
+        const double x_axis[3] = {v[1] * up[2] - v[2] * up[1], v[2] * up[0] - v[0] * up[2], v[0] * up[1] - v[1] * up[0]};
+        for (int q = 0; q < 3; q++) { Rs.R[q] = x_axis[q]; Rs.R[3 + q] = up[q]; Rs.R[6 + q] = v[q]; }
+    }
     TRY(D.upload(&d_pts, pts, (size_t) n * 3));
     TRY(D.upload(&d_proj, projections, (size_t) nvis * 2));
     if (pt_protected) TRY(D.upload(&d_prot, pt_protected, (size_t) n));
     const int gb = (nvis + 255) / 256;
-    if (d_intr) outlier_dist_kernel<true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
-    else outlier_dist_kernel<false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, d_pts, d_proj, estimate_distortion ? 1 : 0, d_dist);
+    const int ud = estimate_distortion ? 1 : 0;
+    if (d_fe) {
+        if (d_intr) outlier_dist_kernel<true, true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, d_fe, Rs, d_pts, d_proj, ud, d_dist);
+        else outlier_dist_kernel<false, true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, d_fe, Rs, d_pts, d_proj, ud, d_dist);
+    } else {
+        if (d_intr) outlier_dist_kernel<true, false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, nullptr, Rs, d_pts, d_proj, ud, d_dist);
+        else outlier_dist_kernel<false, false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, nullptr, Rs, d_pts, d_proj, ud, d_dist);
+    }
     BSFM_KERNEL_CHECK();
 
     // per-camera sorted distances, in the camera-major view (ascending point order within each camera)
@@ -205,7 +251,7 @@ extern "C" int bsfm_reprojection_outliers(int num_pts, int num_cameras, const ch
                                           const char *pt_protected, double *cam_stats, double *obs_dist,
                                           int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
 {
-    return outliers_impl(num_pts, num_cameras, VisSource::mask(vmask), projections, cams, pts, estimate_distortion,
+    return outliers_impl(num_pts, num_cameras, VisSource::mask(vmask), projections, cams, pts, estimate_distortion, 0, 0,
                          min_proj_error_threshold, max_proj_error_threshold, pt_protected, cam_stats, obs_dist, outliers,
                          outlier_errors, cap, global_mean);
 }
@@ -218,6 +264,29 @@ extern "C" int bsfm_reprojection_outliers_crs(int num_pts, int num_cameras, cons
                                               int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
 {
     return outliers_impl(num_pts, num_cameras, VisSource::crs(vis_ptr, vis_cam, nvis), projections, cams, pts,
-                         estimate_distortion, min_proj_error_threshold, max_proj_error_threshold, pt_protected, cam_stats,
+                         estimate_distortion, 0, 0, min_proj_error_threshold, max_proj_error_threshold, pt_protected, cam_stats,
                          obs_dist, outliers, outlier_errors, cap, global_mean);
+}
+
+extern "C" int bsfm_reprojection_outliers_fe(int num_pts, int num_cameras, const char *vmask, const double *projections,
+                                             const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion,
+                                             int optimize_for_fisheye, double min_proj_error_threshold, double max_proj_error_threshold,
+                                             const char *pt_protected, double *cam_stats, double *obs_dist,
+                                             int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
+{
+    return outliers_impl(num_pts, num_cameras, VisSource::mask(vmask), projections, cams, pts, estimate_distortion, 1,
+                         optimize_for_fisheye, min_proj_error_threshold, max_proj_error_threshold, pt_protected, cam_stats, obs_dist,
+                         outliers, outlier_errors, cap, global_mean);
+}
+
+extern "C" int bsfm_reprojection_outliers_crs_fe(int num_pts, int num_cameras, const int32_t *vis_ptr, const int32_t *vis_cam,
+                                                 int nvis, const double *projections, const bsfm_camera_params_t *cams,
+                                                 const bsfm_v3_t *pts, int estimate_distortion, int optimize_for_fisheye,
+                                                 double min_proj_error_threshold, double max_proj_error_threshold,
+                                                 const char *pt_protected, double *cam_stats, double *obs_dist,
+                                                 int32_t *outliers, double *outlier_errors, int cap, double *global_mean)
+{
+    return outliers_impl(num_pts, num_cameras, VisSource::crs(vis_ptr, vis_cam, nvis), projections, cams, pts,
+                         estimate_distortion, 1, optimize_for_fisheye, min_proj_error_threshold, max_proj_error_threshold,
+                         pt_protected, cam_stats, obs_dist, outliers, outlier_errors, cap, global_mean);
 }

@@ -109,8 +109,8 @@ struct Solve {
     double *d_p, *d_pdp, *d_e, *d_enew, *d_camR_a, *d_camR_b, *d_Lmat, *d_linv, *d_da, *d_mu;
     double *const h_mu;
     Scalars *const h_sc;
-    decltype(&residual_kernel<false>) k_residual = nullptr;
-    decltype(&jacobian_kernel<false>) k_jacobian = nullptr;
+    decltype(&residual_kernel<false, false>) k_residual = nullptr;
+    decltype(&jacobian_kernel<false, false>) k_jacobian = nullptr;
     // what the controller ends with (info[], sba_levmar.c:2028-2049)
     double mu = 0.0, eab_inf = 0.0, p_eL2 = 0.0, dp_L2 = DBL_MAX, init_p_eL2 = 0.0, max_diag = DBL_MIN;
     int stop = 0, nfev = 0, njev = 0, nlss = 0, itno = 0;
@@ -132,7 +132,7 @@ struct Solve {
         P.Sdim = Sdim;
     }
     int visibility(const VisSource &vis, const double *x);
-    int upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, const double *p, const double *fixed_pts,
+    int upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, bool fisheye, const double *p, const double *fixed_pts,
                int use_constraints, const bsfm_camera_constraints_t *constraints,
                int use_point_constraints, const bsfm_point_constraints_t *point_constraints);
     int controller(int itmax, int verbose, const double opts[6], bool any_constraints, double *Vout);
@@ -191,8 +191,8 @@ int Solve::visibility(const VisSource &vis, const double *x)
     return D.upload(&P.x, x, (size_t) nobs);
 }
 
-// model, calibrated cameras, constraints, work arrays and the initial parameters
-int Solve::upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, const double *p, const double *fixed_pts,
+// model, calibrated cameras, fisheye cameras, constraints, work arrays and the initial parameters
+int Solve::upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, bool fisheye, const double *p, const double *fixed_pts,
                   int use_constraints, const bsfm_camera_constraints_t *constraints,
                   int use_point_constraints, const bsfm_point_constraints_t *point_constraints)
 {
@@ -210,8 +210,21 @@ int Solve::upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *ini
             TRY(D.upload(&P.intr, h_intr.data(), (size_t) m));
         }
     }
-    k_residual = P.intr ? residual_kernel<true> : residual_kernel<false>;
-    k_jacobian = P.intr ? jacobian_kernel<true> : jacobian_kernel<false>;
+    // the fisheye projection (sfm_project_point2_fisheye, sfm.c:448-492): its table exists only when the call asks for it,
+    // and selects the FE kernels
+    std::vector<CamFisheye> h_fe;
+    if (fisheye) {
+        h_fe.resize(m);
+        for (int j = 0; j < m; j++) h_fe[j] = cam_fisheye(init_params[j]);
+        TRY(D.upload(&P.fe, h_fe.data(), (size_t) m));
+    }
+    if (P.fe) {
+        k_residual = P.intr ? residual_kernel<true, true> : residual_kernel<false, true>;
+        k_jacobian = P.intr ? jacobian_kernel<true, true> : jacobian_kernel<false, true>;
+    } else {
+        k_residual = P.intr ? residual_kernel<true, false> : residual_kernel<false, false>;
+        k_jacobian = P.intr ? jacobian_kernel<true, false> : jacobian_kernel<false, false>;
+    }
     std::vector<char> h_cc; std::vector<double> h_cv, h_cw;
     if (use_constraints) {
         if (!constraints) { set_error("use_constraints set but constraints == NULL"); return BSFM_ERR_ARG; }
@@ -426,9 +439,10 @@ int Solve::export_blocks(double *Vout, double *Sout, double *Uout, double *Wout)
 
 // Shared implementation of the two LM drivers (mot: see Solve).
 // init_params (nullable, m entries): the calibrated-camera fields (known_intrinsics, K_known, k_known) are read.
+// fisheye: project with sfm_project_point2_fisheye; init_params is required then, and its fisheye fields are read too.
 static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon, const VisSource &vis, double *p, int cnp, int pnp,
                        const double *x, const double *covx, int mnp,
-                       const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, int jac_mode,
+                       const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, int fisheye, int jac_mode,
                        int itmax, int verbose, const double opts[6], double info[10],
                        int use_constraints, const bsfm_camera_constraints_t *constraints,
                        int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
@@ -438,6 +452,10 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     TRY(require_device());
     if (n <= 0 || m <= 0 || mcon < 0 || mcon >= m || !vis.present() || !p || !x || !model || !opts || (mot && !fixed_pts)) {
         set_error("bsfm_sba_motstr_levmar_model: bad arguments (n=%d m=%d mcon=%d)", n, m, mcon);
+        return BSFM_ERR_ARG;
+    }
+    if (fisheye && !init_params) {
+        set_error("bsfm_sba_motstr_levmar_model: the fisheye projection reads init_params, which is NULL");
         return BSFM_ERR_ARG;
     }
     if (pnp != 3 || mnp != 2 || cnp < 6 || cnp > 9 || cnp != 6 + (model->est_focal_length ? 1 : 0) + (model->undistort ? 2 : 0)) {
@@ -463,7 +481,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     S.PT.begin(0);
     TRY(S.visibility(vis, x));
     TRY(build_schur_structure(S.P, st, S.D));
-    TRY(S.upload(model, init_params, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints));
+    TRY(S.upload(model, init_params, fisheye != 0, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints));
     S.PT.end();
     S.HM.mark("setup issued");
 
@@ -494,8 +512,22 @@ extern "C" int bsfm_sba_motstr_levmar_model_ki(int n, int m, int mcon, const cha
                                                double *Vout, double *Sout, double *Uout, double *Wout,
                                                const bsfm_camera_params_t *init_params)
 {
-    return levmar_impl(0, nullptr, n, m, mcon, VisSource::mask(vmask), p, cnp, pnp, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
-                       use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout);
+    return levmar_impl(0, nullptr, n, m, mcon, VisSource::mask(vmask), p, cnp, pnp, x, covx, mnp, model, init_params, 0, jac_mode, itmax, verbose,
+                       opts, info, use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout);
+}
+
+extern "C" int bsfm_sba_motstr_levmar_model_fe(int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
+                                               const double *x, const double *covx, int mnp,
+                                               const bsfm_sfm_model_t *model, int jac_mode,
+                                               int itmax, int verbose, const double opts[6], double info[10],
+                                               int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                               int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
+                                               double *Vout, double *Sout, double *Uout, double *Wout,
+                                               const bsfm_camera_params_t *init_params, int optimize_for_fisheye)
+{
+    return levmar_impl(0, nullptr, n, m, mcon, VisSource::mask(vmask), p, cnp, pnp, x, covx, mnp, model, init_params, optimize_for_fisheye,
+                       jac_mode, itmax, verbose, opts, info, use_constraints, constraints, use_point_constraints, point_constraints,
+                       Vout, Sout, Uout, Wout);
 }
 
 extern "C" int bsfm_sba_motstr_levmar_model(int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
@@ -518,8 +550,19 @@ extern "C" int bsfm_sba_mot_levmar_model_ki(int n, int m, int mcon, const char *
                                             int use_constraints, const bsfm_camera_constraints_t *constraints,
                                             const bsfm_camera_params_t *init_params)
 {
-    return levmar_impl(1, points, n, m, mcon, VisSource::mask(vmask), p, cnp, 3, x, covx, mnp, model, init_params, jac_mode, itmax, verbose, opts, info,
-                       use_constraints, constraints, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
+    return levmar_impl(1, points, n, m, mcon, VisSource::mask(vmask), p, cnp, 3, x, covx, mnp, model, init_params, 0, jac_mode, itmax, verbose,
+                       opts, info, use_constraints, constraints, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
+}
+
+extern "C" int bsfm_sba_mot_levmar_model_fe(int n, int m, int mcon, const char *vmask, double *p, int cnp,
+                                            const double *x, const double *covx, int mnp,
+                                            const bsfm_sfm_model_t *model, const double *points, int jac_mode,
+                                            int itmax, int verbose, const double opts[6], double info[10],
+                                            int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                            const bsfm_camera_params_t *init_params, int optimize_for_fisheye)
+{
+    return levmar_impl(1, points, n, m, mcon, VisSource::mask(vmask), p, cnp, 3, x, covx, mnp, model, init_params, optimize_for_fisheye,
+                       jac_mode, itmax, verbose, opts, info, use_constraints, constraints, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
 }
 
 extern "C" int bsfm_sba_mot_levmar_model(int n, int m, int mcon, const char *vmask, double *p, int cnp,
@@ -598,11 +641,11 @@ static int run_sfm_impl(int num_pts, int num_cameras, int ncons, const VisSource
                         bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
                         int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
                         double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
-                        double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
+                        double *Vout, double *Sout, double *Uout, double *Wout, double *info_out, bool fisheye_entry)
 {
     clear_error();
     if (fix_points && (Vout || Sout || Uout || Wout)) { set_error("bsfm_run_sfm: fix_points=1 has no V/S/U/W export (nor has the reference, sfm.c:843-856)"); return BSFM_ERR_UNSUPPORTED; }
-    if (optimize_for_fisheye) { set_error("bsfm_run_sfm: optimize_for_fisheye=1 is outside the GPU path"); return BSFM_ERR_UNSUPPORTED; }
+    if (optimize_for_fisheye && !fisheye_entry) { set_error("bsfm_run_sfm: optimize_for_fisheye=1 is outside this entry; bsfm_run_sfm_fe runs it"); return BSFM_ERR_UNSUPPORTED; }
     if (est_focal_length && const_focal_length) { set_error("bsfm_run_sfm: const_focal_length is not implemented (nor in the reference, sfm.c:518-521)"); return BSFM_ERR_UNSUPPORTED; }
     if (num_pts <= 0 || num_cameras <= 0 || !vis.present() || !projections || !init_camera_params || !init_pts) {
         set_error("bsfm_run_sfm: bad arguments"); return BSFM_ERR_ARG;
@@ -687,11 +730,11 @@ static int run_sfm_impl(int num_pts, int num_cameras, int ncons, const VisSource
     int rc;
     if (fix_points)     // sfm.c:843-849: motion-only BA, the points come from init_pts and stay as they are
         rc = levmar_impl(1, params.data() + num_camera_params, num_pts, num_cameras, ncons, vis, params.data(), cnp, 3, projections,
-                         nullptr, 2, &model, init_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                         nullptr, 2, &model, init_camera_params, optimize_for_fisheye, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
                          use_constraints, use_constraints ? constraints.data() : nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
     else
         rc = levmar_impl(0, nullptr, num_pts, num_cameras, ncons, vis, params.data(), cnp, 3, projections, nullptr, 2,
-                         &model, init_camera_params, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                         &model, init_camera_params, optimize_for_fisheye, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
                          use_constraints, use_constraints ? constraints.data() : nullptr,
                          use_point_constraints, use_point_constraints ? point_constraints.data() : nullptr,
                          Vout, Sout, Uout, Wout);
@@ -749,7 +792,7 @@ extern "C" int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask
 {
     return run_sfm_impl(num_pts, num_cameras, ncons, VisSource::mask(vmask), projections, est_focal_length, const_focal_length,
                         undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints, use_point_constraints,
-                        pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2, Vout, Sout, Uout, Wout, info_out);
+                        pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2, Vout, Sout, Uout, Wout, info_out, false);
 }
 
 extern "C" int bsfm_run_sfm_crs(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
@@ -762,5 +805,30 @@ extern "C" int bsfm_run_sfm_crs(int num_pts, int num_cameras, int ncons, const i
     return run_sfm_impl(num_pts, num_cameras, ncons, VisSource::crs(vis_ptr, vis_cam, nvis), projections, est_focal_length,
                         const_focal_length, undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints,
                         use_point_constraints, pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2,
-                        Vout, Sout, Uout, Wout, info_out);
+                        Vout, Sout, Uout, Wout, info_out, false);
+}
+
+extern "C" int bsfm_run_sfm_fe(int num_pts, int num_cameras, int ncons, char *vmask, double *projections,
+                               int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
+                               bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                               int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
+                               double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                               double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
+{
+    return run_sfm_impl(num_pts, num_cameras, ncons, VisSource::mask(vmask), projections, est_focal_length, const_focal_length,
+                        undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints, use_point_constraints,
+                        pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2, Vout, Sout, Uout, Wout, info_out, true);
+}
+
+extern "C" int bsfm_run_sfm_crs_fe(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                                   double *projections, int est_focal_length, int const_focal_length, int undistort,
+                                   int explicit_camera_centers, bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                                   int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
+                                   double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                                   double *Vout, double *Sout, double *Uout, double *Wout, double *info_out)
+{
+    return run_sfm_impl(num_pts, num_cameras, ncons, VisSource::crs(vis_ptr, vis_cam, nvis), projections, est_focal_length,
+                        const_focal_length, undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints,
+                        use_point_constraints, pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2,
+                        Vout, Sout, Uout, Wout, info_out, true);
 }

@@ -144,6 +144,99 @@ def ba_scene_known_intrinsics(num_cameras=20, num_points=2000, views_per_point=5
     }
 
 
+def fisheye_map(u, params):
+    """sfm_fisheye_distort (lib/sfm-driver/sfm.c:426-446) of pinhole points u (N x 2) with per-point fisheye_params
+    (N x 5: f_cx, f_cy, f_rad, f_angle, f_focal), in the reference's operation order -> pixels (N x 2)"""
+    cx, cy, rad, fang, F = (params[:, q] for q in range(5))
+    r = np.sqrt(u[:, 0] * u[:, 0] + u[:, 1] * u[:, 1])
+    angle = 180.0 * np.arctan(r / F) / np.pi
+    rnew = rad * angle / (0.5 * fang)
+    return np.stack([u[:, 0] * (rnew / r) + cx, u[:, 1] * (rnew / r) + cy], 1)
+
+
+def ba_scene_fisheye(num_cameras=20, num_points=2000, views_per_point=5, seed=2468, ordinary_fraction=0.25, known_fraction=0.0,
+                     pixel_noise=0.5, pt_noise=0.02, cam_noise=0.01, f_noise=0.01, focal=800.0, min_radius=5.0):
+    """A ba_scene measured through the reference's fisheye projection (sfm_project_point2_fisheye, lib/sfm-driver/
+    sfm.c:448-492): the pinhole without the radial step, then, for the fisheye cameras, sfm_fisheye_distort with the
+    camera's f_cx, f_cy, f_rad, f_angle, f_focal, plus N(0, pixel_noise^2).  A seeded `ordinary_fraction` of the cameras are
+    not fisheye; a seeded `known_fraction` are calibrated (known_intrinsics, K_known / k_known as in
+    ba_scene_known_intrinsics) and may be fisheye too.  Points are redrawn until every pinhole projection lies at least
+    `min_radius` px from the principal point (the mapping is 0/0 there).  Adds fisheye [m] int8 and fisheye_params [m,5]
+    (and known / K_known / k_known with known_fraction) to the ba_scene dict; fe_kwargs(scene) passes them on."""
+    rng = np.random.default_rng(seed)
+    m, n, L = num_cameras, num_points, views_per_point
+    ang = 2.0 * np.pi * np.arange(m) / m
+    c = np.stack([6.0 * np.cos(ang), 0.3 * np.sin(3 * ang), 6.0 * np.sin(ang)], 1)
+    R = np.zeros((m, 3, 3))
+    for j in range(m):
+        z = c[j] / np.linalg.norm(c[j])
+        xax = np.cross(np.array([0.0, 1.0, 0.0]), z); xax /= np.linalg.norm(xax)
+        R[j] = np.stack([xax, np.cross(z, xax), z], 0)
+    fisheye = np.ones(m, np.int8)
+    n_ord = int(round(ordinary_fraction * m))
+    if n_ord:
+        fisheye[rng.choice(m, size=n_ord, replace=False)] = 0
+    F = focal * (1.0 + 0.05 * rng.standard_normal(m))
+    fang = rng.uniform(160.0, 200.0, m)
+    rad = F * (0.5 * fang) * (np.pi / 180.0) * rng.uniform(0.9, 1.1, m)     # near-unit scale at the image centre
+    params = np.stack([rng.uniform(-20.0, 20.0, m), rng.uniform(-20.0, 20.0, m), rad, fang, F], 1)
+    known = np.zeros(m, np.int8)
+    n_kn = int(round(known_fraction * m))
+    if n_kn:
+        known[rng.choice(m, size=n_kn, replace=False)] = 1
+    K_known = np.zeros((m, 3, 3))
+    K_known[:, 0, 0] = focal * (1.0 + 0.05 * rng.standard_normal(m))
+    K_known[:, 0, 1] = rng.uniform(-3.0, 3.0, m)
+    K_known[:, 0, 2] = rng.uniform(-25.0, 25.0, m)
+    K_known[:, 1, 1] = K_known[:, 0, 0] * (1.0 + 0.01 * rng.standard_normal(m))
+    K_known[:, 1, 2] = rng.uniform(-25.0, 25.0, m)
+    K_known[:, 2, 2] = 1.0
+    k_known = np.stack([rng.uniform(-0.12, -0.04, m), rng.uniform(0.01, 0.04, m), rng.uniform(-2e-3, 2e-3, m),
+                        rng.uniform(-2e-3, 2e-3, m), rng.uniform(-4e-3, 4e-3, m)], 1)
+    vmask = np.zeros((n, m), np.int8)
+    step = max(m // L, 1)
+    starts = (np.arange(n) * 7) % m
+    for k in range(L):
+        vmask[np.arange(n), (starts + k * step) % m] = 1
+    pi, cj = np.nonzero(vmask)
+    pts = rng.uniform(-1.0, 1.0, size=(n, 3))
+    while True:
+        Pc = np.einsum("oij,oj->oi", R[cj], pts[pi] - c[cj])
+        u = -Pc[:, :2] * focal / Pc[:, 2:3]
+        kn = known[cj] != 0
+        if kn.any():
+            from .bundle import project_known
+            u[kn] = project_known(Pc[kn], K_known[cj[kn]].reshape(-1, 9), k_known[cj[kn]])
+        near = np.unique(pi[np.hypot(u[:, 0], u[:, 1]) < min_radius])
+        if not len(near):
+            break
+        pts[near] = rng.uniform(-1.0, 1.0, size=(len(near), 3))
+    fe = fisheye[cj] != 0
+    proj = u.copy()
+    proj[fe] = fisheye_map(u[fe], params[cj[fe]])
+    proj = proj + pixel_noise * rng.standard_normal(proj.shape)
+    f0 = np.where(known != 0, K_known[:, 0, 0], focal)
+    scene = {
+        "vmask": vmask, "projections": np.ascontiguousarray(proj),
+        "gt_pts": pts, "gt_c": c, "gt_R": R.reshape(m, 9).copy(), "gt_f": f0.copy(),
+        "R": R.reshape(m, 9).copy(),
+        "c": c + cam_noise * rng.standard_normal(c.shape),
+        "f": f0 * (1.0 + f_noise * rng.standard_normal(m)),
+        "k": np.zeros((m, 2)),
+        "pts": pts + pt_noise * rng.standard_normal(pts.shape),
+        "fisheye": fisheye, "fisheye_params": params,
+    }
+    if n_kn:
+        scene.update(known=known, K_known=K_known.reshape(m, 9).copy(), k_known=k_known)
+    return scene
+
+
+def fe_kwargs(scene):
+    """the camera keywords of a fisheye scene (fisheye, fisheye_params, and the calibration when it has one) for run_sfm /
+    call_run_sfm / reprojection_outliers; empty for a scene without them"""
+    return {k: scene[k] for k in ("fisheye", "fisheye_params", "known", "K_known", "k_known") if k in scene}
+
+
 def crs_scene(scene):
     """a copy of a scene dict whose visibility is CRS instead of the dense vmask: vis_ptr [n+1] int32 (point i's
     observations are vis_ptr[i]..vis_ptr[i+1]) and vis_cam [nvis] int32 (ascending camera within a point), i.e.

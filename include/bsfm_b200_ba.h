@@ -125,14 +125,38 @@ int bsfm_sba_mot_levmar_model_ki(int n, int m, int mcon, const char *vmask, doub
                                  int use_constraints, const bsfm_camera_constraints_t *constraints,
                                  const bsfm_camera_params_t *init_params);
 
+/* The two _ki solvers above with the fisheye projection of run_sfm's optimize_for_fisheye (sfm_project_point2_fisheye
+ * and its _mot twin, lib/sfm-driver/sfm.c:448-501).  optimize_for_fisheye == 0: exactly the _ki entries.  With 1, every
+ * camera projects through the pinhole (focal-only, or K_known / k_known for a calibrated camera) WITHOUT the radial step,
+ * so with undistort the k1, k2 columns of the Jacobian are exactly zero and only camera constraints move them; then a
+ * camera with fisheye != 0 maps the pinhole point u to u * rnew / |u| + (f_cx, f_cy), rnew = f_rad * angle / (f_angle / 2),
+ * angle = 180 atan(|u| / f_focal) / pi (sfm_fisheye_distort, :426-446).  A point on a fisheye camera's principal axis
+ * gives NaN, as in the reference (it ends the solve through stop 7).  init_params (host memory) is required with 1; its
+ * fisheye, f_cx, f_cy, f_rad, f_angle, f_focal fields are read besides the calibration.  Both Jacobian modes cover it. */
+int bsfm_sba_motstr_levmar_model_fe(int n, int m, int mcon, const char *vmask, double *p, int cnp, int pnp,
+                                    const double *x, const double *covx, int mnp,
+                                    const bsfm_sfm_model_t *model, int jac_mode,
+                                    int itmax, int verbose, const double opts[6], double info[10],
+                                    int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                    int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
+                                    double *Vout, double *Sout, double *Uout, double *Wout,
+                                    const bsfm_camera_params_t *init_params, int optimize_for_fisheye);
+int bsfm_sba_mot_levmar_model_fe(int n, int m, int mcon, const char *vmask, double *p, int cnp,
+                                 const double *x, const double *covx, int mnp,
+                                 const bsfm_sfm_model_t *model, const double *points, int jac_mode,
+                                 int itmax, int verbose, const double opts[6], double info[10],
+                                 int use_constraints, const bsfm_camera_constraints_t *constraints,
+                                 const bsfm_camera_params_t *init_params, int optimize_for_fisheye);
+
 /* == run_sfm (lib/sfm-driver/sfm.h:68-86): same arguments, same in/out semantics
  * (init_camera_params and init_pts are overwritten with the solution, sfm.c:876-929; prints
  * "[run_sfm] Number of iterations" / "info[6]" like sfm.c:872-873), plus `info_out` (nullable,
  * 10 doubles) and an int return (0 or negative error) which the void reference lacks.
  * fix_points == 1 runs the motion-only solver (sfm.c:843-849; init_pts untouched).  Cameras with
  * known_intrinsics != 0 project through their K_known / k_known (see bsfm_sba_motstr_levmar_model_ki), which
- * run_sfm neither packs nor changes.  GPU path covers optimize_for_fisheye == 0 and const_focal_length == 0;
- * anything else returns BSFM_ERR_UNSUPPORTED.                                                   */
+ * run_sfm neither packs nor changes.  This entry covers optimize_for_fisheye == 0 and const_focal_length == 0;
+ * anything else returns BSFM_ERR_UNSUPPORTED (callers may rely on that to route fisheye work elsewhere);
+ * bsfm_run_sfm_fe runs optimize_for_fisheye == 1.                                              */
 int bsfm_run_sfm(int num_pts, int num_cameras, int ncons, char *vmask, double *projections,
                  int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
                  bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
@@ -163,6 +187,23 @@ int bsfm_run_sfm_crs(int num_pts, int num_cameras, int ncons, const int32_t *vis
                      double point_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
                      double *Vout, double *Sout, double *Uout, double *Wout, double *info_out);
 
+/* bsfm_run_sfm and bsfm_run_sfm_crs, same arguments, honouring optimize_for_fisheye: with 1 the solver projects like
+ * sfm_project_point2_fisheye (see bsfm_sba_motstr_levmar_model_fe; fix_points selects the _mot twin, sfm.c:829-856),
+ * reading each camera's fisheye fields from init_camera_params, which it leaves as they are.  With 0 these are
+ * bit-identical to the entries they extend, fisheye cameras included (their fisheye byte is not read then).        */
+int bsfm_run_sfm_fe(int num_pts, int num_cameras, int ncons, char *vmask, double *projections,
+                    int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
+                    bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                    int use_constraints, int use_point_constraints, bsfm_v3_t *points_constraints,
+                    double point_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                    double *Vout, double *Sout, double *Uout, double *Wout, double *info_out);
+int bsfm_run_sfm_crs_fe(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                        double *projections, int est_focal_length, int const_focal_length, int undistort,
+                        int explicit_camera_centers, bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                        int use_constraints, int use_point_constraints, bsfm_v3_t *points_constraints,
+                        double point_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                        double *Vout, double *Sout, double *Uout, double *Wout, double *info_out);
+
 /* The reprojection statistics / outlier pass BundlerApp::RunSFM_SBA runs after every run_sfm on the same
  * vmask / projections / cameras / points (src/Bundle.cpp:659-856), as one call (SURVEY.md 8f row 1):
  *   dist(obs)   = || sfm_project_rd(camera, point, estimate_distortion, explicit centres) - measurement ||  (:721-754)
@@ -172,7 +213,8 @@ int bsfm_run_sfm_crs(int num_pts, int num_cameras, int ncons, const int32_t *vis
  *                 "constrained point" rule, :801-806); the reported error is the distance in the first (lowest
  *                 index) camera that flags the point, like the reference's first-found rule (:809-821)
  * cameras: the `R`, `t` (= centre), `f`, `k` fields of run_sfm's output are read, and for cameras with known_intrinsics
- *   != 0 also K_known and k_known (sfm.c:339-357, then the radial step with f and k).  fisheye cameras are refused.
+ *   != 0 also K_known and k_known (sfm.c:339-357, then the radial step with f and k).  fisheye cameras are refused
+ *   (bsfm_reprojection_outliers_fe takes them).
  * cam_stats (nullable): num_cameras x 5 = { #observations, mean distance, median (iround(0.5 n)-th), med80, thresh }
  * obs_dist  (nullable): one distance per observation in the order of `projections`
  * outliers / outlier_errors: up to `cap` entries, ordered by (first flagging camera, point index) -- the
@@ -194,6 +236,24 @@ int bsfm_reprojection_outliers_crs(int num_pts, int num_cameras, const int32_t *
                                    int estimate_distortion, double min_proj_error_threshold, double max_proj_error_threshold,
                                    const char *pt_protected, double *cam_stats, double *obs_dist,
                                    int32_t *outliers, double *outlier_errors, int cap, double *global_mean);
+
+/* The two outlier entries above with an optimize_for_fisheye argument after estimate_distortion; they accept fisheye
+ * cameras either way, as the reference does.  With 1, a camera with fisheye != 0 passes its sfm_project_rd projection
+ * through ImageData::DistortPoint (src/Bundle.cpp:746-751, ImageData.cpp:1129-1169): the ray (x, y, -f_focal), rotated
+ * by GetRotationFromSpherical(-pi/2, pi/2) (computed on the host with the C library's cos / sin), is re-projected and
+ * mapped like sfm_fisheye_distort with RAD2DEG(a) = a * (180 / pi); a ray whose rotated z is <= 0 keeps the undistorted
+ * projection.  With 0 every camera is projected as an ordinary (or calibrated) one.                                   */
+int bsfm_reprojection_outliers_fe(int num_pts, int num_cameras, const char *vmask, const double *projections,
+                                  const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion,
+                                  int optimize_for_fisheye, double min_proj_error_threshold, double max_proj_error_threshold,
+                                  const char *pt_protected, double *cam_stats, double *obs_dist,
+                                  int32_t *outliers, double *outlier_errors, int cap, double *global_mean);
+int bsfm_reprojection_outliers_crs_fe(int num_pts, int num_cameras, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                                      const double *projections, const bsfm_camera_params_t *cams, const bsfm_v3_t *pts,
+                                      int estimate_distortion, int optimize_for_fisheye,
+                                      double min_proj_error_threshold, double max_proj_error_threshold,
+                                      const char *pt_protected, double *cam_stats, double *obs_dist,
+                                      int32_t *outliers, double *outlier_errors, int cap, double *global_mean);
 
 /* == sba_Axb_Chol (lib/sba-1.5/sba_lapack.c:374-485, called at sba_levmar.c:1343): x = A^-1 B for a symmetric
  * positive definite m x m matrix (dpotrf + dpotrs in the reference).  A, B, x: host or device pointers; A and B are

@@ -9,13 +9,15 @@
  * A GPU solver cannot call an opaque host callback per observation (SURVEY.md H5), so the callbacks are RECOGNISED:
  *   proj == sfm_project_point3      (sfm.c:503-552)  with adata -> sfm_global_t  ->  bsfm_sba_motstr_levmar_model
  *   proj == sfm_project_point3_mot  (sfm.c:554-561)                              ->  bsfm_sba_mot_levmar_model
+ *   proj == sfm_project_point2_fisheye / _mot (sfm.c:448-501, what run_sfm passes with optimize_for_fisheye)
+ *                                   -> bsfm_sba_motstr_levmar_model_fe / bsfm_sba_mot_levmar_model_fe with optimize_for_fisheye = 1
  *   expert drivers: func == bsfm_sba_motstr_Qs / bsfm_sba_mot_Qs (the marker the simple drivers of this library pass,
  *   the counterpart of the static sba_motstr_Qs of sba_levmar_wrap.c:73-104) with projac == NULL (finite differences,
  *   what run_sfm uses: sfm.c:821).
  * Anything else -- a foreign projection, an analytic projac, covx != NULL -- fails LOUDLY: message on stderr and
  * SBA_ERROR (-1), the reference's own error convention.  There is no CPU fallback.
- * In the reference sfm_project_point3 is `static`; libsfmdrv_b200.so exports it (with a host implementation, so that
- * code which calls it directly keeps working) precisely so that its address can be recognised. */
+ * In the reference these callbacks are `static`; libsfmdrv_b200.so exports them (with a host implementation, so that
+ * code which calls them directly keeps working) precisely so that their addresses can be recognised. */
 #ifndef BSFM_B200_SBA_H
 #define BSFM_B200_SBA_H
 #include "bsfm_b200_ba.h"
@@ -35,6 +37,9 @@ typedef struct {
 /* == sfm_project_point3 / sfm_project_point3_mot (sfm.c:503-561): host evaluation of one projection */
 void sfm_project_point3(int j, int i, double *aj, double *bi, double *xij, void *adata);
 void sfm_project_point3_mot(int j, int i, double *aj, double *xij, void *adata);
+/* == sfm_project_point2_fisheye / sfm_project_point2_fisheye_mot (sfm.c:448-501): host evaluation of one projection */
+void sfm_project_point2_fisheye(int j, int i, double *aj, double *bi, double *xij, void *adata);
+void sfm_project_point2_fisheye_mot(int j, int i, double *aj, double *xij, void *adata);
 
 struct sba_crsm;
 /* markers passed by the simple drivers of libsba_b200 to its expert drivers (never executed by the GPU solver) */

@@ -28,7 +28,7 @@ void bsfm_sba_mot_Qs_fdjac(double *p, struct sba_crsm *idxij, int *rcidxs, int *
 
 static int unsupported(const char *fn, const char *what)
 {
-    fprintf(stderr, "SBA/b200: %s(): %s -- only the sfm-driver projection (sfm_project_point3, finite-difference Jacobian, covx == NULL) "
+    fprintf(stderr, "SBA/b200: %s(): %s -- only the sfm-driver projections (sfm_project_point3, sfm_project_point2_fisheye, finite-difference Jacobian, covx == NULL) "
                     "runs on the GPU and there is no CPU fallback\n", fn, what);
     return SBA_ERROR_RC;
 }
@@ -83,17 +83,18 @@ int sba_motstr_levmar_x(const int n, const int m, const int mcon, char *vmask, d
     int rc;
     if (func != bsfm_sba_motstr_Qs || !wd) return unsupported(fn, "unknown `func` callback");
     if (fjac != bsfm_sba_motstr_Qs_fdjac || wd->projac) return unsupported(fn, "analytic Jacobian callback");
-    if (wd->proj != sfm_project_point3) return unsupported(fn, "unknown `proj` callback");
+    if (wd->proj != sfm_project_point3 && wd->proj != sfm_project_point2_fisheye) return unsupported(fn, "unknown `proj` callback");
     if (covx) return unsupported(fn, "covx != NULL");
     if (wd->cnp != cnp || wd->pnp != pnp || wd->mnp != mnp) return unsupported(fn, "inconsistent block sizes");
     if (itmax == 0) return unsupported(fn, "itmax == 0 (Jacobian verification mode)");
     rc = model_from_globals(fn, (const bsfm_sfm_global_t *) wd->adata, m, cnp, &model, &R_init, &f_fixed);
     if (rc) return rc;
     /* opts really has 6 entries for the Bundler build of sba (it reads opts[5], sba_levmar.c:610) */
-    /* calibrated cameras: sfm_project_point3 reads known_intrinsics / K_known / k_known from the same init_params */
-    rc = bsfm_sba_motstr_levmar_model_ki(n, m, mcon, vmask, p, cnp, pnp, x, NULL, mnp, &model, BSFM_BA_JAC_FD, itmax, verbose, opts, info,
+    /* calibrated cameras: sfm_project_point3 reads known_intrinsics / K_known / k_known from the same init_params, and
+     * sfm_project_point2_fisheye the fisheye fields too */
+    rc = bsfm_sba_motstr_levmar_model_fe(n, m, mcon, vmask, p, cnp, pnp, x, NULL, mnp, &model, BSFM_BA_JAC_FD, itmax, verbose, opts, info,
                                          use_constraints, constraints, use_point_constraints, point_constraints, Vout, Sout, Uout, Wout,
-                                         ((const bsfm_sfm_global_t *) wd->adata)->init_params);
+                                         ((const bsfm_sfm_global_t *) wd->adata)->init_params, wd->proj == sfm_project_point2_fisheye);
     free(R_init); free(f_fixed);
     return finish(fn, rc);
 }
@@ -144,15 +145,15 @@ int sba_mot_levmar_x(const int n, const int m, const int mcon, char *vmask, doub
     int rc;
     if (func != bsfm_sba_mot_Qs || !wd) return unsupported(fn, "unknown `func` callback");
     if (fjac != bsfm_sba_mot_Qs_fdjac || wd->projac) return unsupported(fn, "analytic Jacobian callback");
-    if (wd->proj != sfm_project_point3_mot) return unsupported(fn, "unknown `proj` callback");
+    if (wd->proj != sfm_project_point3_mot && wd->proj != sfm_project_point2_fisheye_mot) return unsupported(fn, "unknown `proj` callback");
     if (covx) return unsupported(fn, "covx != NULL");
     if (itmax == 0) return unsupported(fn, "itmax == 0 (Jacobian verification mode)");
     g = (const bsfm_sfm_global_t *) wd->adata;
     rc = model_from_globals(fn, g, m, cnp, &model, &R_init, &f_fixed);
     if (rc) return rc;
     if (!g->points) { free(R_init); free(f_fixed); return unsupported(fn, "adata->points is NULL"); }
-    rc = bsfm_sba_mot_levmar_model_ki(n, m, mcon, vmask, p, cnp, x, NULL, mnp, &model, (const double *) g->points, BSFM_BA_JAC_FD, itmax, verbose,
-                                      opts, info, use_constraints, constraints, g->init_params);
+    rc = bsfm_sba_mot_levmar_model_fe(n, m, mcon, vmask, p, cnp, x, NULL, mnp, &model, (const double *) g->points, BSFM_BA_JAC_FD, itmax, verbose,
+                                      opts, info, use_constraints, constraints, g->init_params, wd->proj == sfm_project_point2_fisheye_mot);
     free(R_init); free(f_fixed);
     return finish(fn, rc);
 }
