@@ -23,7 +23,6 @@ namespace ba {
 int chol_solve_dataflow(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *x, Scalars *sc, bool *used);
 
 constexpr int NB = 32;
-constexpr int CHOL_LARGE_MIN = 1536;     // systems above this size are throughput-bound: 256-column panel path
 
 // ---- small systems, one launch per 32-column step ---------------------------------------------------
 // Every CTA redundantly factors the 32x32 diagonal block (one warp, rows in registers, pivots and

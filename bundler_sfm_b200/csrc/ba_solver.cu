@@ -580,7 +580,12 @@ extern "C" int bsfm_sba_mot_levmar_model(int n, int m, int mcon, const char *vma
 // iscolmaj == 1; a symmetric matrix reads the same in both orders, so the flag changes nothing else here).
 // Returns 1 on success, 0 when a leading minor is not positive definite (the reference's return values), < 0 on a
 // library error.  `reps` > 1 repeats the factorisation on a fresh copy of A; *ms_out = device time per repetition.
-static int axb_chol_impl(const double *A, const double *B, double *x, int m, int reps, float *ms_out)
+// `out` (bsfm_sba_Axb_Chol_factor): what the factorisation left behind, copied out whether or not it succeeded.
+struct CholOutputs {
+    double *L, *linv, *xinv;
+    int *fail_code;
+};
+static int axb_chol_impl(const double *A, const double *B, double *x, int m, int reps, float *ms_out, const CholOutputs *out = nullptr)
 {
     clear_error();
     TRY(require_device());
@@ -596,6 +601,8 @@ static int axb_chol_impl(const double *A, const double *B, double *x, int m, int
     BSFM_CUDA_TRY(cudaMemcpyAsync(d_src, A, mm * sizeof(double), cudaMemcpyDefault, st));
     BSFM_CUDA_TRY(cudaMemcpyAsync(d_src + mm, B, (size_t) m * sizeof(double), cudaMemcpyDefault, st));
     BSFM_CUDA_TRY(cudaMemsetAsync(d_sc, 0, sizeof(Scalars), st));
+    // every path writes the lower triangle of Lmat only: zeroed first, its upper part comes back as the zeros it was given
+    if (out && out->L) BSFM_CUDA_TRY(cudaMemsetAsync(d_L, 0, (mm + m) * sizeof(double), st));
     cudaEvent_t e0, e1;
     BSFM_CUDA_TRY(cudaEventCreate(&e0)); BSFM_CUDA_TRY(cudaEventCreate(&e1));
     float total = 0.f;
@@ -613,9 +620,23 @@ static int axb_chol_impl(const double *A, const double *B, double *x, int m, int
     if (ms_out) *ms_out = total / reps;
     Scalars h;
     BSFM_CUDA_TRY(cudaMemcpy(&h, d_sc, sizeof h, cudaMemcpyDeviceToHost));
+    if (out) {
+        if (out->fail_code) *out->fail_code = h.chol_fail;
+        if (out->L) BSFM_CUDA_TRY(cudaMemcpy(out->L, d_L, mm * sizeof(double), cudaMemcpyDefault));
+        const size_t nlinv = (size_t) ((m + LNB - 1) / LNB) * LNB * LNB;
+        if (out->linv) BSFM_CUDA_TRY(cudaMemcpy(out->linv, d_linv, nlinv * sizeof(double), cudaMemcpyDefault));
+        // the large path (ba_chol_large.cu) keeps the panel inverses right behind the 32 x 32 ones
+        if (out->xinv && m > CHOL_LARGE_MIN)
+            BSFM_CUDA_TRY(cudaMemcpy(out->xinv, d_linv + nlinv, (size_t) ((m + LNBO - 1) / LNBO) * LNBO * LNBO * sizeof(double), cudaMemcpyDefault));
+    }
     if (h.chol_fail) return 0;
     BSFM_CUDA_TRY(cudaMemcpy(x, d_x, (size_t) m * sizeof(double), cudaMemcpyDefault));
     return 1;
+}
+extern "C" int bsfm_sba_Axb_Chol_factor(const double *A, const double *B, double *x, int m, double *L, double *linv, double *xinv, int *fail_code)
+{
+    const CholOutputs out = {L, linv, xinv, fail_code};
+    return axb_chol_impl(A, B, x, m, 1, nullptr, &out);
 }
 extern "C" int bsfm_sba_Axb_Chol(const double *A, const double *B, double *x, int m, int iscolmaj)
 {

@@ -265,6 +265,21 @@ int bsfm_sba_Axb_Chol(const double *A, const double *B, double *x, int m, int is
 /* the same solve repeated `reps` times on a fresh copy of A; *ms_per_solve = mean device time (CUDA events) of one
  * factorisation + both triangular solves (measurement entry used by bench.py and the tests)                          */
 int bsfm_sba_Axb_Chol_timed(const double *A, const double *B, double *x, int m, int reps, float *ms_per_solve);
+/* Test / diagnostic entry: the solve of bsfm_sba_Axb_Chol (same launches, same return values and x), plus what it
+ * computed on the way.  Every output may be NULL; all are copied out even when the factorisation fails.
+ *   L          m x m row-major: the lower triangle of the factor.  Every path writes only that triangle of a zeroed
+ *              matrix, so the upper part comes back as +0.
+ *   linv       ceil(m/32) blocks of 32 x 32 row-major, block k = (L_kk)^-1 of the k-th diagonal 32-block (lower
+ *              triangular, zero above the diagonal), written by chol_step_kernel (m <= 32 and 641..1536), the
+ *              dataflow kernel (33..640 and the last panels of larger systems) or chol_diag_kernel (the other panels of
+ *              m > 1536).  In a partial last block only rows and columns < m mod 32 are the inverse.
+ *   xinv       m > 1536 only (ignored otherwise): ceil(m/256) blocks of 256 x 256 row-major, block p = (L_pp)^-T of the
+ *              p-th diagonal 256-block (upper triangular), which the back substitution multiplies with.  In a partial
+ *              last block only rows and columns < m mod 256 are written.
+ *   fail_code  the raw failure word of the factorisation: 0 none, 1 a non-positive or non-finite pivot, 2 a word of the
+ *              dataflow kernel (csrc/ba_chol_dataflow.cu) that never arrived.  Any nonzero value returns 0.       */
+int bsfm_sba_Axb_Chol_factor(const double *A, const double *B, double *x, int m, double *L, double *linv, double *xinv,
+                             int *fail_code);
 
 /* Per-kernel-class device timing of the large-system Cholesky (systems > 1536 unknowns), for roofline reporting:
  * bsfm_ba_chol_profile(1) resets the counters of the calling thread and records CUDA events around every launch of

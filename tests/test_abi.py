@@ -76,6 +76,12 @@ def test_compute_fails_loudly_without_gpu():
     off = np.array([0, 4], np.int64)
     h = lib.bsfm_keydb_create(k.ctypes.data, off.ctypes.data, 1)
     assert not h
+    A, L = np.eye(4), np.zeros((4, 4))
+    b, x, linv = np.ones(4), np.zeros(4), np.zeros((1, 32, 32))
+    fail = ctypes.c_int(-7)
+    rc = lib.bsfm_sba_Axb_Chol_factor(ctypes.c_void_p(A.ctypes.data), ctypes.c_void_p(b.ctypes.data), ctypes.c_void_p(x.ctypes.data), 4,
+                                      ctypes.c_void_p(L.ctypes.data), ctypes.c_void_p(linv.ctypes.data), None, ctypes.byref(fail))
+    assert rc < 0 and fail.value == -7 and not x.any()
 
 
 def test_pair_count_helper():
