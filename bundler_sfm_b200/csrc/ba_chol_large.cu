@@ -163,7 +163,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) chol_diag_kernel(double *A, dou
 // fragment row, and the XOR spreads the eight lanes of every quarter warp (rows g, g + 1 for even g; t = 0..3) over the
 // eight 16-byte bank groups: the fragment loads are free of bank conflicts without padding
 // (tests/test_chol_trailing_swizzle.py enumerates them).
-constexpr int SY_BT = 128, SY_BK = 32, SY_KCH = LNBO / SY_BK;      // tile, K chunk, chunks per panel
+constexpr int SY_BT = CHOL_TILE, SY_BK = 32, SY_KCH = LNBO / SY_BK;      // tile, K chunk, chunks per panel
 constexpr int SY_BLOCK = SY_BT * SY_BK;                             // doubles per operand stage (32 KB)
 constexpr int SY_STAGES = 3;
 constexpr int SY_CONSUMERS = 8, SY_THREADS = 32 * (SY_CONSUMERS + 4);      // two consumer warpgroups + the producer's
@@ -173,7 +173,7 @@ constexpr int SY_PRODUCER_REGS = 40, SY_CONSUMER_REGS = 232;
 // The shared list of a launch's nonzero row blocks: 16-bit entries behind two int counts.  A launch with more row blocks
 // (n > 16 K) keeps every tile.  The list is kept this short on purpose: the same kernel with 2 KB or 8 KB more shared memory
 // (even without the skip) returned wrong factors of dense systems from n ~ 3800 on (H100, cause not found, DESIGN.md §8).
-constexpr int SY_MAX_RB = 128;
+constexpr int SY_MAX_RB = CHOL_MAX_RB;
 constexpr size_t SY_SMEM = (size_t) SY_STAGES * 2 * SY_BLOCK * sizeof(double) + 2 * SY_STAGES * 8 + 2 * sizeof(int) + SY_MAX_RB * sizeof(uint16_t);
 __device__ __forceinline__ size_t syrk_img_index(int q, int c)
 {
@@ -196,7 +196,7 @@ static size_t syrk_img_doubles(int n) { return (size_t) ((n + 1 - LNBO + SY_BT -
 // for them whenever the diagonal block factored (finite L_kk and Z).  Its image rows are written too: the trailing update
 // reads them when the other 64 rows of their 128-row block are nonzero.
 constexpr int SLAB_NONZERO = 1, SLAB_NONFINITE = 2;
-constexpr int TR_ROWS = 64;
+constexpr int TR_ROWS = CHOL_SLAB;
 constexpr int TR_LDX = LNBO + 4;       // pitch = 4 (mod 16) doubles: conflict-free DMMA fragment loads
 constexpr int TR_LDB = LNB + 4;
 constexpr int TR_NLB = LNBO / LNB;      // blocks staged per sub-step: L_s0 .. L_s,s-1 and Z_ss
@@ -648,13 +648,14 @@ struct CholProfile {
     size_t used = 0;
     struct Span { int cls; cudaEvent_t a, b; };
     std::vector<Span> spans;
+    std::vector<size_t> open;     // spans begun and not yet ended, innermost last (the look-ahead's diagonal block nests in an update)
     cudaEvent_t get() { if (used == pool.size()) { cudaEvent_t e; cudaEventCreate(&e); pool.push_back(e); } return pool[used++]; }
-    void begin(int cls, cudaStream_t st) { if (!on) return; Span sp{cls, get(), get()}; cudaEventRecord(sp.a, st); spans.push_back(sp); }
-    void end(cudaStream_t st) { if (!on) return; cudaEventRecord(spans.back().b, st); launches[spans.back().cls]++; }
+    void begin(int cls, cudaStream_t st) { if (!on) return; Span sp{cls, get(), get()}; cudaEventRecord(sp.a, st); open.push_back(spans.size()); spans.push_back(sp); }
+    void end(cudaStream_t st) { if (!on) return; const Span &sp = spans[open.back()]; open.pop_back(); cudaEventRecord(sp.b, st); launches[sp.cls]++; }
     void collect()
     {
         for (auto &sp : spans) { cudaEventSynchronize(sp.b); float t = 0; cudaEventElapsedTime(&t, sp.a, sp.b); ms[sp.cls] += t; }
-        spans.clear(); used = 0;
+        spans.clear(); open.clear(); used = 0;
     }
 };
 thread_local CholProfile g_prof;
@@ -718,7 +719,7 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
     // The last panels are latency-bound (a serial diagonal chain per panel that no trailing update hides any more): once the
     // remaining matrix fits the one-launch dataflow factorisation (ba_chol_dataflow.cu, <= 640), it takes over in place -- same
     // factor blocks, same 32 x 32 inverses, so the batched panel inverses and the back substitution below do not notice.
-    static const int tail_max = []() { const char *e = getenv("BSFM_BA_CHOL_TAIL"); return e ? atoi(e) : 640; }();
+    static const int tail_max = []() { const char *e = getenv("BSFM_BA_CHOL_TAIL"); return e ? atoi(e) : CHOL_TAIL_MAX; }();
     auto tail_fits = [&](int kk) { return kk > 0 && kk < n && n - kk <= tail_max && n - kk > 2 * LNB; };
     for (int k0 = 0; k0 < n; k0 += LNBO) {
         const int nb = std::min(LNBO, n - k0);
@@ -764,11 +765,12 @@ int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *li
                 BSFM_KERNEL_CHECK();
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_col, st));
                 BSFM_CUDA_TRY(cudaStreamWaitEvent(side.st, side.e_col, 0));
+                g_prof.begin(0, side.st);
                 chol_diag_kernel<<<1, DG_THREADS, DG_SMEM_DOUBLES * sizeof(double), side.st>>>(A, Lmat, ld, n, k1, linv_ws, sc);
                 BSFM_KERNEL_CHECK();
+                g_prof.end(side.st);
                 BSFM_CUDA_TRY(cudaEventRecord(side.e_diag, side.st));
                 diag_done = true;
-                if (g_prof.on) g_prof.launches[0]++;
                 update(k2, n, sms - 1);
             } else {
                 update(k1, n, sms);

@@ -13,6 +13,10 @@ struct Scalars;
 constexpr int LNB = 32;          // sub-block
 constexpr int LNBO = 256;        // outer panel
 constexpr int CHOL_LARGE_MIN = 1536;     // systems above this size are throughput-bound: 256-column panel path
+// geometry of the large path's zero-block skip (ba_chol_large.cu), shared with the camera order that feeds it (ba_order.cu):
+// the panel solve flags 64-row slabs, the trailing update keeps 128 x 128 tiles from a list of at most 128 row blocks, and the
+// dataflow kernel takes over once at most CHOL_TAIL_MAX columns remain (BSFM_BA_CHOL_TAIL)
+constexpr int CHOL_SLAB = 64, CHOL_TILE = 128, CHOL_MAX_RB = 128, CHOL_TAIL_MAX = 640;
 int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *xinv_ws, double *x, Scalars *sc);
 // doubles of linear-solver workspace behind the 32 x 32 inverses: back-substitution scratch (small path) or the 256 x 256 panel inverses (large path)
 constexpr int DF_MAX_N = 24 * LNB;       // largest system the dataflow path (ba_chol_dataflow.cu) takes: it needs (n + 1) x n doubles more

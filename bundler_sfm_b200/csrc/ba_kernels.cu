@@ -843,7 +843,7 @@ __global__ void __launch_bounds__(128) schur_final_kernel(Problem P)
         for (int u = 0; u < 4; u++) { acc[0] += v[u][0]; acc[1] += v[u][1]; acc[2] += v[u][2]; accE += v[u][3]; }
     }
     const int Sdim = P.Sdim;
-    const int jr = (j - P.mcon) * cnp, kr = (k - P.mcon) * cnp;
+    const int jr = cam_block(P, j) * cnp, kr = cam_block(P, k) * cnp;      // S is symmetric: both triangles are written
 #pragma unroll
     for (int rep = 0; rep < 3; rep++) {
         const int q = lane + 32 * rep;
@@ -884,7 +884,7 @@ __global__ void backsub_kernel(Problem P, const double *da)
     const int cnp = P.M.cnp;
     if (i < P.m * cnp) {
         const int j = i / cnp;
-        P.dp[i] = (j < P.mcon) ? 0.0 : da[i - P.mcon * cnp];
+        P.dp[i] = (j < P.mcon) ? 0.0 : da[cam_block(P, j) * cnp + (i - j * cnp)];
     }
     if (i >= P.n) return;
     double w0 = 0.0, w1 = 0.0, w2 = 0.0;
@@ -892,7 +892,7 @@ __global__ void backsub_kernel(Problem P, const double *da)
         const int j = P.obs_cam[o];
         if (j < P.mcon) continue;
         const double *Wo = P.W + (size_t) o * cnp * 3;
-        const double *d = da + (size_t) (j - P.mcon) * cnp;
+        const double *d = da + (size_t) cam_block(P, j) * cnp;
         double s0 = 0.0, s1 = 0.0, s2 = 0.0;
         for (int jj = 0; jj < cnp; jj++) {
             const double dv = d[jj];

@@ -127,6 +127,7 @@ struct Problem {
     int nchunks;
     const int *chunk_off;      // nblocks+1: first chunk of every block
     double *schur_part;        // nchunks * SCHUR_PART_STRIDE
+    const int *cam_pos;        // m - mcon: block position of free camera j in S and da (camera_order, ba_order.cu), or null: j - mcon
     // data
     const double *x;       // 2*nvis measurements
     const double *R_init;  // m*9
@@ -158,6 +159,9 @@ struct Problem {
     const CamIntrinsics *intr;  // m entries, or null when no camera is calibrated (then only the KI = false kernels run)
     const CamFisheye *fe;       // m entries, or null without the fisheye projection (then only the FE = false kernels run)
 };
+
+// block position of free camera j (>= mcon) in S, E and the dense solution
+__device__ __forceinline__ int cam_block(const Problem &P, int j) { return P.cam_pos ? P.cam_pos[j - P.mcon] : j - P.mcon; }
 
 // launch with the programmatic-stream-serialization attribute (PDL): the launch latency of a kernel overlaps
 // the tail of its predecessor; every kernel launched this way calls cudaGridDependencySynchronize() before it

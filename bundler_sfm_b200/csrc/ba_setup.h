@@ -85,5 +85,13 @@ int build_visibility(const VisSource &src, int n, int m, cudaStream_t st, Device
 // Schur structure of P's visibility: fills P.nblocks, blk_key, blk_start, tuples, nchunks, chunk_off and schur_part
 int build_schur_structure(Problem &P, cudaStream_t st, DeviceArena &D);
 
+// Camera order of the reduced camera system (ba_order.cu, bsfm_ba_camera_order): pos[j - mcon] = block position of free
+// camera j; scores[0] / [1] = tiles the large Cholesky's trailing update keeps in the natural / RCM order.  Returns 1 when
+// RCM is taken, 0 when the natural order is kept (then pos is the identity).
+int camera_order(int m, int mcon, int cnp, const uint32_t *keys, int nblocks, std::vector<int> &pos, int64_t scores[2]);
+// Applies it to P (sets P.cam_pos) when the system takes the large Cholesky path and RCM wins; BSFM_BA_CAMERA_ORDER=0 keeps
+// the natural order.  Reads P.blk_key back to the host (one synchronisation of st).
+int apply_camera_order(Problem &P, int cnp, cudaStream_t st, DeviceArena &D);
+
 }  // namespace ba
 }  // namespace bsfm

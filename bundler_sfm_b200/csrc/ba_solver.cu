@@ -430,6 +430,7 @@ int Solve::export_blocks(double *Vout, double *Sout, double *Uout, double *Wout)
     }
     *h_mu = 0.0;
     BSFM_CUDA_TRY(cudaMemcpyAsync(d_mu, h_mu, sizeof(double), cudaMemcpyHostToDevice, st));
+    P.cam_pos = nullptr;      // S goes out in the caller's camera order, whichever order the solves factored it in
     TRY(schur(true));
     BSFM_CUDA_TRY(cudaMemcpyAsync(Sout, P.S, (size_t) Sdim * Sdim * sizeof(double), cudaMemcpyDefault, st));   // symmetric: transpose == itself (:2017-2025)
     return BSFM_OK;
@@ -481,6 +482,8 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     S.PT.begin(0);
     TRY(S.visibility(vis, x));
     TRY(build_schur_structure(S.P, st, S.D));
+    if (!mot) TRY(apply_camera_order(S.P, cnp, st, S.D));      // large systems: S in the order that skips most of the factorisation
+    S.HM.mark("Schur structure + camera order");
     TRY(S.upload(model, init_params, fisheye != 0, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints));
     S.PT.end();
     S.HM.mark("setup issued");

@@ -286,9 +286,20 @@ int bsfm_sba_Axb_Chol_factor(const double *A, const double *B, double *x, int m,
  * the following solves; bsfm_ba_chol_profile_read returns accumulated ms / launch counts for
  * [0] diagonal-block factorisation  [1] panel solve  [2] trailing update  [3] back substitution,
  * and the fp64 FLOPs of the trailing update (2 per multiply-add of the lower triangle).  Call it after the solves
- * have completed.                                                                                                   */
+ * have completed.  [0] includes the diagonal blocks the look-ahead factors on its side stream, next to the trailing update
+ * (their time overlaps [2]).                                                                                        */
 int bsfm_ba_chol_profile(int enable);
 int bsfm_ba_chol_profile_read(float ms[4], int launches[4], double *fp64_flops);
+
+/* Camera order of a motion+structure solve whose reduced camera system takes the large Cholesky path
+ * ((m - mcon) * cnp > 1536 unknowns); host only.  blk_key[0 .. nblocks): the Schur blocks j * m + k (j <= k; cameras
+ * j, k >= mcon share a point; diagonal keys may be present).  Scores the natural camera order and reverse Cuthill-McKee
+ * by the 128 x 128 tiles the trailing update keeps over the whole factorisation (scores[0] natural, scores[1] RCM), from
+ * the symbolic block structure of the factor, and takes RCM when it keeps at most 3/4 of the natural order's tiles.
+ * cam_pos[j - mcon] receives the block position of free camera j (m - mcon entries; the identity when the natural order
+ * is kept).  Smaller systems keep the natural order, unscored (scores 0).  Returns 1 for RCM, 0 for the natural order,
+ * < 0 on bad arguments.  The solver applies the order unless BSFM_BA_CAMERA_ORDER=0.                                   */
+int bsfm_ba_camera_order(int m, int mcon, int cnp, const uint32_t *blk_key, int nblocks, int32_t *cam_pos, int64_t scores[2]);
 
 /* Per-phase device time (ms, CUDA events) of the last solve of this thread:
  * [0] setup (H2D, CSR, Schur structure)  [1] residual/Jacobian/U/V/W  [2] Schur S assembly
