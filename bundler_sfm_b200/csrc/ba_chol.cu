@@ -304,13 +304,13 @@ __global__ void __launch_bounds__(512) chol_backsolve_blocked_kernel(const doubl
     }
 }
 
-// symmetric S (both triangles filled by the Schur kernel) + E in row n.  x receives the solution.
+// symmetric S (both triangles filled by the Schur kernel) + E in row n.  x receives the solution.  band: see chol_solve_large.
 // Lmat: (n+1) x n factor matrix (out of place: A's panel columns stay readable during a step).
 // linv_ws: ceil(n/32) * 1024 doubles (+ n doubles of back-substitution workspace behind it).
-int chol_solve(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *x, Scalars *sc)
+int chol_solve(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *x, Scalars *sc, const CholBand *band)
 {
     const int nbk = (n + NB - 1) / NB;
-    if (n > CHOL_LARGE_MIN) return chol_solve_large(st, A, Lmat, n, linv_ws, linv_ws + (size_t) nbk * NB * NB, x, sc);
+    if (n > CHOL_LARGE_MIN) return chol_solve_large(st, A, Lmat, n, linv_ws, linv_ws + (size_t) nbk * NB * NB, x, sc, band);
     if (n > LNB) {      // small systems: one co-resident dataflow launch per factorisation (ba_chol_dataflow.cu)
         bool used = false;
         int rc = chol_solve_dataflow(st, A, Lmat, n, linv_ws, x, sc, &used);

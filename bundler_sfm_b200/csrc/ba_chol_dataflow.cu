@@ -1,5 +1,6 @@
 // ba_chol_dataflow.cu -- dense SPD factorisation of SMALL reduced camera systems (n <= 640; config 2: 50 cameras -> 450) as ONE
-// co-resident launch per factorisation; also finishes the last panels of large systems in place (ba_chol_large.cu).
+// co-resident launch per factorisation; also finishes the last panels of large systems in place (ba_chol_large.cu), and factors
+// large systems with a narrow row envelope whole (chol_band_kernel, below).
 // Reference: dpotrf inside sba_Axb_Chol, lib/sba-1.5/sba_lapack.c:429.
 //
 // Small systems are bound by the chain of n sequential pivots and by L2 round trips, not by FLOPs.  The
@@ -30,6 +31,9 @@ namespace ba {
 
 constexpr int DF_THREADS = 256;
 constexpr long long DF_SPIN_LIMIT = 400000;      // polls of one L2 round trip each: a lost flag costs well under a second, never a hang
+// The band kernel's workers may start their first tile hundreds of steps into the factorisation and wait for all of them:
+// its bound grows with the step count (a step takes ~11 us; this allows well over a millisecond of polls per step)
+constexpr long long DF_SPIN_PER_STEP = 4000;
 
 // ---- data that is its own "ready" flag ----
 // Everything that travels between CTAs (Z_kk blocks, finished tiles) is written exactly once per solve into memory the host
@@ -51,7 +55,7 @@ __device__ __forceinline__ bool df_pending(double v) { return __double_as_longlo
 // Fetch NE elements per thread: element i of this thread comes from src(i) (nullptr: not part of the tile, takes fill(i)) and is
 // handed to put(i, value).  Re-reads the words that are still pending (bounded).
 template <int NE, class Src, class Put>
-__device__ __forceinline__ void df_fetch(Src src, Put put, Scalars *sc)
+__device__ __forceinline__ void df_fetch(Src src, Put put, Scalars *sc, long long spin_limit = DF_SPIN_LIMIT)
 {
     double v[NE];
     unsigned pend = 0;
@@ -70,7 +74,7 @@ __device__ __forceinline__ void df_fetch(Src src, Put put, Scalars *sc)
                 if (!df_pending(v[i])) pend &= ~(1u << i);
             }
         }
-        if (++spins > DF_SPIN_LIMIT) { sc->chol_fail = 2; break; }
+        if (++spins > spin_limit) { sc->chol_fail = 2; break; }
         if (pend) __nanosleep(32);
     }
 #pragma unroll
@@ -311,6 +315,331 @@ __global__ void __launch_bounds__(DF_THREADS, 1) chol_dataflow_kernel(const doub
         }
         __syncthreads();                    // the X buffers are free again
     }
+}
+
+// ================= the same dataflow over the envelope of a large banded system =================
+// chol_band_kernel factors a system whose rows have a narrow envelope (CholBandPlan, ba_chol_large.cuh) in one cooperative
+// launch; the tiles outside the envelope are zero in L and never touched.
+//   CTA 0        the diagonal chain of chol_dataflow_kernel, except that the sub-diagonal block (k+1, k) may lie outside the
+//                envelope (it is zero then: no look-ahead update), and the sender warp 4 forms the right-hand-side segment
+//                y_k = (row n, block k) Z_kk^T at every step
+//   CTAs 1..W    the tiles of the host's schedule, at most two at a time in registers: a tile enters its slot from A at its
+//                first update step and leaves through the publish buffer after its last.  A worker fetches panel blocks and
+//                Z_kk only at the steps where one of its tiles takes an update.  The owner of a diagonal tile (rb, rb) writes
+//                block (rb, k) of L at every step k it takes, which covers every envelope block below the sub-diagonal.
+//   publish      envelope-packed: tile (rb, cb) is the 32 x 32 block number toff[rb] + cb - env[rb] (row pitch 32).  A tile that
+//                took no update from a worker is read from A by its consumers.
+__global__ void __launch_bounds__(DF_THREADS, 1) chol_band_kernel(const double *A, double *Lout, int ld, int n, double *linv_all /* pre-filled */,
+                                                                  double *Pub /* pre-filled */, const CholBand B, long long spin_limit, Scalars *sc)
+{
+    __shared__ __align__(16) double tiles[5][LNB][TP];      // CTA 0: L_kk, next diagonal tile, X, Z, W;  workers: Z, 2 x (X_r, X_c)
+    __shared__ __align__(16) double yrow[8][TP];            // CTA 0: the right-hand-side segment in row 0 (rows 1..7 stay zero)
+    __shared__ double dinv[LNB];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g = lane >> 2, tg = lane & 3;
+    const int nbk = (n + LNB - 1) / LNB;
+    const int *env = B.env;
+
+    auto rows_of = [&](int rb) { return (rb == nbk) ? 1 : min(LNB, n - rb * LNB); };
+    auto rbase_of = [&](int rb) { return (rb == nbk) ? n : rb * LNB; };
+    // finished envelope tile (x, c): element (r, q) is p[r * lds + q]
+    struct TileSrc { const double *p; int lds; };
+    auto tile_src = [&](int x, int c) -> TileSrc {
+        const bool worked = max(env[x], env[c]) <= ((x == c) ? c - 2 : c - 1);
+        if (worked) return {Pub + ((size_t) (B.toff[x] + c - env[x]) << 10), LNB};
+        return {A + (size_t) rbase_of(x) * ld + (size_t) c * LNB, ld};
+    };
+
+    if (blockIdx.x == 0) {
+        double (*Lc)[TP] = tiles[0], (*Ln)[TP] = tiles[1];
+        double (*Xr)[TP] = tiles[2], (*Zs)[TP] = tiles[3], (*Ws)[TP] = tiles[4];
+        {
+            const int nb0 = min(LNB, n);
+            for (int e = tid; e < LNB * LNB; e += DF_THREADS) {
+                const int r = e >> 5, c = e & 31;
+                Lc[r][c] = (r < nb0 && c <= r) ? A[(size_t) r * ld + c] : ((r == c) ? 1.0 : 0.0);
+                Zs[r][c] = 0.0;
+            }
+            for (int e = tid; e < 8 * TP; e += DF_THREADS) yrow[e / TP][e % TP] = 0.0;
+        }
+        __syncthreads();
+        for (int k = 0; k < nbk; k++) {
+            const int k0 = k * LNB, nb = min(LNB, n - k0);
+            const bool last = (k + 1 == nbk);
+            const bool sub = !last && env[k + 1] <= k;          // block (k+1, k) lies in the envelope
+            const int rrows = last ? 0 : rows_of(k + 1), rbase = (k + 1) * LNB;
+            if (warp >= 4) {
+                // ---- senders ----
+                DF_BAR(7, 192);                                 // potf2 and inverse done
+                for (int e = tid - 128; e < LNB * LNB; e += 128) st_strong(&linv_all[(size_t) k * LNB * LNB + e], ((e & 31) <= (e >> 5)) ? Zs[e >> 5][e & 31] : 0.0);
+                for (int e = tid - 128; e < LNB * LNB; e += 128) {
+                    const int r = e >> 5, c = e & 31;
+                    if (r < nb && c <= r) Lout[(size_t) (k0 + r) * ld + (k0 + c)] = Lc[r][c];
+                }
+                if (warp == 4) {                                // forward substitution: y_k, after Z_kk has gone out
+                    const TileSrc y = tile_src(nbk, k);
+                    df_fetch<1>([&](int) -> const double * { return (lane < nb) ? y.p + lane : nullptr; },
+                                [&](int, double v) { yrow[0][lane] = v; }, sc, spin_limit);
+                    __syncwarp();
+                    warp_rows_times_ZT(yrow, 0, Zs, lane);
+                    __syncwarp();
+                    if (lane < nb) Lout[(size_t) n * ld + (k0 + lane)] = yrow[0][lane];
+                }
+            } else {
+                if (warp == 0) {
+                    const bool bad = warp_potf2_32_tc(Lc, dinv, lane, true);
+                    if (bad && lane == 0) sc->chol_fail = 1;
+                    __syncwarp();
+                    DF_ARRIVE(7, 192);
+                } else if (warp == 1) {
+                    warp_tile_inverse(Lc, dinv, Zs, Ws, lane);
+                    DF_ARRIVE(7, 192);
+                } else if (!last) {
+                    const TileSrc xs = sub ? tile_src(k + 1, k) : TileSrc{A, ld};
+                    const TileSrc ds = tile_src(k + 1, k + 1);
+                    const int t64 = tid - 64;
+#pragma unroll 1
+                    for (int e0 = 0; e0 < LNB * LNB; e0 += 64 * 8) {
+                        if (sub)
+                            df_fetch<8>([&](int i) -> const double * { const int e = e0 + t64 + 64 * i, r = e >> 5, c = e & 31;
+                                                                       return (r < rrows && c < nb) ? xs.p + (size_t) r * xs.lds + c : nullptr; },
+                                        [&](int i, double v) { const int e = e0 + t64 + 64 * i; Xr[e >> 5][e & 31] = v; }, sc, spin_limit);
+                        df_fetch<8>([&](int i) -> const double * { const int e = e0 + t64 + 64 * i, r = e >> 5, c = e & 31;
+                                                                   return (r < rrows && c <= r) ? ds.p + (size_t) r * ds.lds + c : nullptr; },
+                                    [&](int i, double v) { const int e = e0 + t64 + 64 * i, r = e >> 5, c = e & 31;
+                                                           Ln[r][c] = (r < rrows && c <= r) ? v : ((r == c) ? 1.0 : 0.0); }, sc, spin_limit);
+                    }
+                }
+                DF_BAR(8, 128);                                 // factor, inverse and look-ahead inputs are in shared memory
+                if (sub) warp_rows_times_ZT(Xr, 8 * warp, Zs, lane);
+                DF_BAR(8, 128);
+                if (sub) {
+                    for (int e = tid; e < LNB * LNB; e += 128) {
+                        const int r = e >> 5, c = e & 31;
+                        if (r < rrows && c < nb) Lout[(size_t) (rbase + r) * ld + (k0 + c)] = Xr[r][c];
+                    }
+                    for (int t = warp; t < 10; t += 4) {       // lower 8 x 8 tiles (ri, cj) of the next diagonal tile
+                        int ri = 0, rem = t;
+                        while (rem > ri) { rem -= ri + 1; ri++; }
+                        const int cj = rem;
+                        double c0 = 0.0, c1 = 0.0;
+#pragma unroll
+                        for (int ks = 0; ks < LNB; ks += 4) tile_dmma(c0, c1, Xr[8 * ri + g][ks + tg], Xr[8 * cj + g][ks + tg]);
+                        double2 cur = *reinterpret_cast<const double2 *>(&Ln[8 * ri + g][8 * cj + 2 * tg]);
+                        cur.x -= c0; cur.y -= c1;
+                        *reinterpret_cast<double2 *>(&Ln[8 * ri + g][8 * cj + 2 * tg]) = cur;
+                    }
+                }
+            }
+            __syncthreads();
+            double (*tmp)[TP] = Lc; Lc = Ln; Ln = tmp;
+        }
+        return;
+    }
+
+    // ================= workers: the host's schedule, two register slots =================
+    double (*Zs)[TP] = tiles[0];
+    const int w = (int) blockIdx.x - 1;
+    constexpr int NONE = 0x7fffffff;
+    int next[2], stop[2], trb[2], tcb[2], klast[2], knext[2];
+    double cur[2][2][2];
+    auto take = [&](int s) {        // the slot's next tile (knext = its first update step), its values from A
+        trb[s] = tcb[s] = 0; klast[s] = -1; knext[s] = NONE;
+        if (next[s] < stop[s]) {
+            const int t = B.sched[next[s]];
+            trb[s] = t >> 16; tcb[s] = t & 0xffff;
+            knext[s] = max(env[trb[s]], env[tcb[s]]);
+            klast[s] = (trb[s] == tcb[s]) ? tcb[s] - 2 : tcb[s] - 1;
+        }
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int t = warp * 2 + i, r = 8 * (t >> 2) + g, c = 8 * (t & 3) + 2 * tg;
+            cur[s][i][0] = cur[s][i][1] = 0.0;
+            if (knext[s] != NONE) {
+                const int rrows = rows_of(trb[s]), crows = rows_of(tcb[s]);
+                const double *src = &A[(size_t) (rbase_of(trb[s]) + r) * ld + (tcb[s] * LNB + c)];
+                if (r < rrows && c < crows) cur[s][i][0] = src[0];
+                if (r < rrows && c + 1 < crows) cur[s][i][1] = src[1];
+            }
+        }
+    };
+#pragma unroll
+    for (int s = 0; s < 2; s++) {
+        next[s] = B.sptr[2 * w + s]; stop[s] = B.sptr[2 * w + s + 1];
+        take(s);
+    }
+    while (true) {
+        const int k = min(knext[0], knext[1]);
+        if (k == NONE) break;
+        const int k0 = k * LNB, nb = min(LNB, n - k0);
+        // (a) the panel blocks of the tiles updated at this step: finished with step k - 1
+#pragma unroll
+        for (int s = 0; s < 2; s++) {
+            if (knext[s] != k) continue;
+            double (*Xr)[TP] = tiles[1 + 2 * s], (*Xc)[TP] = tiles[2 + 2 * s];
+            const int rrows = rows_of(trb[s]), crows = rows_of(tcb[s]);
+            const TileSrc rs = tile_src(trb[s], k);
+            df_fetch<4>([&](int i) -> const double * { const int e = tid + DF_THREADS * i, r = e >> 5, c = e & 31;
+                                                       return (r < rrows && c < nb) ? rs.p + (size_t) r * rs.lds + c : nullptr; },
+                        [&](int i, double v) { const int e = tid + DF_THREADS * i; Xr[e >> 5][e & 31] = v; }, sc, spin_limit);
+            if (trb[s] != tcb[s]) {
+                const TileSrc cs = tile_src(tcb[s], k);
+                df_fetch<4>([&](int i) -> const double * { const int e = tid + DF_THREADS * i, r = e >> 5, c = e & 31;
+                                                           return (r < crows && c < nb) ? cs.p + (size_t) r * cs.lds + c : nullptr; },
+                            [&](int i, double v) { const int e = tid + DF_THREADS * i; Xc[e >> 5][e & 31] = v; }, sc, spin_limit);
+            }
+        }
+        // (b) Z_kk
+        df_fetch<4>([&](int i) -> const double * { return &linv_all[(size_t) k * LNB * LNB + tid + DF_THREADS * i]; },
+                    [&](int i, double v) { const int e = tid + DF_THREADS * i; Zs[e >> 5][e & 31] = v; }, sc, spin_limit);
+        __syncthreads();
+        // (c) X <- X Z^T: up to 16 eight-row strips, two per warp
+#pragma unroll
+        for (int j = 0; j < 2; j++) {
+            const int which = (warp >> 2) & 1, strip = warp & 3;
+            if (knext[j] != k || (which == 1 && trb[j] == tcb[j])) continue;
+            warp_rows_times_ZT(tiles[1 + 2 * j + which], 8 * strip, Zs, lane);
+        }
+        __syncthreads();
+#pragma unroll
+        for (int s = 0; s < 2; s++) {
+            if (knext[s] != k) continue;
+            const double (*Xr)[TP] = tiles[1 + 2 * s];
+            const bool dg = (trb[s] == tcb[s]);
+            const double (*XC)[TP] = dg ? tiles[1 + 2 * s] : tiles[2 + 2 * s];
+            const int rrows = rows_of(trb[s]), crows = rows_of(tcb[s]), rbase = rbase_of(trb[s]);
+            // (d) tile -= X_r X_c^T
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                const int t = warp * 2 + i, ri = t >> 2, cj = t & 3;
+                double a0 = 0.0, a1 = 0.0;
+#pragma unroll
+                for (int ks = 0; ks < LNB; ks += 4) tile_dmma(a0, a1, Xr[8 * ri + g][ks + tg], XC[8 * cj + g][ks + tg]);
+                cur[s][i][0] -= a0; cur[s][i][1] -= a1;
+            }
+            // (e) finished: into the publish buffer, once (the words are their own flags)
+            if (k == klast[s]) {
+                double *dst = Pub + ((size_t) (B.toff[trb[s]] + tcb[s] - env[trb[s]]) << 10);
+#pragma unroll
+                for (int i = 0; i < 2; i++) {
+                    const int t = warp * 2 + i, r = 8 * (t >> 2) + g, c = 8 * (t & 3) + 2 * tg;
+                    if (r < rrows && c < crows && (!dg || c <= r)) st_strong(&dst[r * LNB + c], cur[s][i][0]);
+                    if (r < rrows && c + 1 < crows && (!dg || c + 1 <= r)) st_strong(&dst[r * LNB + c + 1], cur[s][i][1]);
+                }
+            }
+            // (f) a diagonal tile's owner writes block (rb, k) of the factor (read by the back substitution only)
+            if (dg) {
+                for (int e = tid; e < LNB * LNB; e += DF_THREADS) {
+                    const int r = e >> 5, c = e & 31;
+                    if (r < rrows && c < nb) Lout[(size_t) (rbase + r) * ld + (k0 + c)] = Xr[r][c];
+                }
+            }
+        }
+        __syncthreads();                    // the X buffers are free again
+#pragma unroll
+        for (int s = 0; s < 2; s++) {
+            if (knext[s] != k) continue;
+            if (k == klast[s]) { next[s]++; take(s); }
+            else knext[s] = k + 1;
+        }
+    }
+}
+
+// Back substitution L^T x = y over the envelope, one CTA: y (row n of the factor) in shared memory; step kb reads the columns
+// [32 env[kb], 32 kb) of its 32 factor rows only.  Same arithmetic per step as chol_backsolve_blocked_kernel.
+__global__ void __launch_bounds__(512) chol_backsolve_band_kernel(const double *L, int ld, int n, const double *Linv_all, const int *env, double *x)
+{
+    extern __shared__ double ys[];      // n
+    __shared__ double xk[LNB];
+    __shared__ double Li[LNB][LNB + 1];
+    const int tid = threadIdx.x;
+    const double *yrow = L + (size_t) n * ld;
+    for (int c = tid; c < n; c += 512) ys[c] = yrow[c];
+    const int nbk = (n + LNB - 1) / LNB;
+    // the inverse block and this thread's column of the factor rows of step kb - 1 are fetched one step ahead
+    double z0, z1, l[LNB];
+    {
+        const int kb = nbk - 1, k0 = kb * LNB, nb = min(LNB, n - k0), c = LNB * env[kb] + tid;
+        z0 = Linv_all[(size_t) kb * LNB * LNB + tid]; z1 = Linv_all[(size_t) kb * LNB * LNB + 512 + tid];
+#pragma unroll
+        for (int r = 0; r < LNB; r++) l[r] = (c < k0 && r < nb) ? L[(size_t) (k0 + r) * ld + c] : 0.0;
+    }
+    for (int kb = nbk - 1; kb >= 0; kb--) {
+        const int k0 = kb * LNB, nb = min(LNB, n - k0), e0 = LNB * env[kb];
+        Li[tid >> 5][tid & 31] = z0;
+        Li[16 + (tid >> 5)][tid & 31] = z1;
+        if (kb > 0) { z0 = Linv_all[(size_t) (kb - 1) * LNB * LNB + tid]; z1 = Linv_all[(size_t) (kb - 1) * LNB * LNB + 512 + tid]; }
+        __syncthreads();
+        // x_k = L_kk^-T y_k : 8 lanes per output, 4 terms each, shuffle-reduced
+        if (tid < 256) {
+            const int o = tid >> 3, part = tid & 7;
+            double sacc = 0.0;
+#pragma unroll
+            for (int u = 0; u < 4; u++) { const int r = part * 4 + u; if (r >= o && r < nb) sacc = fma(Li[r][o], ys[k0 + r], sacc); }
+            sacc += __shfl_xor_sync(0xffffffffu, sacc, 1);
+            sacc += __shfl_xor_sync(0xffffffffu, sacc, 2);
+            sacc += __shfl_xor_sync(0xffffffffu, sacc, 4);
+            if (part == 0) { xk[o] = sacc; if (o < nb) x[k0 + o] = sacc; }
+        }
+        __syncthreads();
+        if (e0 + tid < k0) {
+            double sacc = 0.0;
+#pragma unroll
+            for (int r = 0; r < LNB; r++) sacc = fma(l[r], xk[r], sacc);
+            ys[e0 + tid] -= sacc;
+        }
+        for (int c = e0 + tid + 512; c < k0; c += 512) {      // envelopes wider than 512 columns: 16 rows at a time
+            double sacc = 0.0;
+#pragma unroll 1
+            for (int r0 = 0; r0 < LNB; r0 += 16) {
+                double lv[16];
+#pragma unroll
+                for (int r = 0; r < 16; r++) lv[r] = (r0 + r < nb) ? L[(size_t) (k0 + r0 + r) * ld + c] : 0.0;
+#pragma unroll
+                for (int r = 0; r < 16; r++) sacc = fma(lv[r], xk[r0 + r], sacc);
+            }
+            ys[c] -= sacc;
+        }
+        if (kb > 0) {                       // rows of step kb - 1 (a full block)
+            const int k1 = k0 - LNB, c = LNB * env[kb - 1] + tid;
+#pragma unroll
+            for (int r = 0; r < LNB; r++) l[r] = (c < k1) ? L[(size_t) (k1 + r) * ld + c] : 0.0;
+        }
+    }
+}
+
+int chol_band_factor(cudaStream_t st, const double *A, double *Lmat, int n, double *linv_ws, const CholBand &B, Scalars *sc)
+{
+    const int nbk = (n + LNB - 1) / LNB;
+    if ((size_t) B.ntile > chol_band_capacity_tiles(n) || n > CHOL_BAND_MAX_N || B.workers < 1) {
+        set_error("chol_band_factor: the plan of n = %d does not fit the workspace", n);
+        return BSFM_ERR_ARG;
+    }
+    // the Z blocks and the packed publish buffer right behind them (in the panel path's xinv area, unused here) are pre-filled
+    // with the "not yet" pattern in one memset
+    double *pub = linv_ws + (size_t) nbk * LNB * LNB;
+    BSFM_CUDA_TRY(cudaMemsetAsync(linv_ws, 0xFF, ((size_t) nbk + B.ntile) * LNB * LNB * sizeof(double), st));
+    long long spin_limit = DF_SPIN_LIMIT + (long long) nbk * DF_SPIN_PER_STEP;
+    int ld = n;
+    CholBand b = B;
+    void *args[] = {&A, &Lmat, &ld, &n, &linv_ws, &pub, &b, &spin_limit, &sc};
+    BSFM_CUDA_TRY(cudaLaunchCooperativeKernel((const void *) chol_band_kernel, dim3(1 + B.workers), dim3(DF_THREADS), args, 0, st));
+    count_launch();
+    return BSFM_OK;
+}
+
+int chol_band_backsolve(cudaStream_t st, const double *Lmat, int n, const double *linv_ws, const CholBand &B, double *x)
+{
+    int dev = 0;
+    BSFM_CUDA_TRY(cudaGetDevice(&dev));
+    static std::atomic<int> attr_set[64];
+    if (dev >= 0 && dev < 64 && !attr_set[dev].load()) {
+        BSFM_CUDA_TRY(cudaFuncSetAttribute(chol_backsolve_band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (CHOL_BAND_MAX_N * sizeof(double))));
+        attr_set[dev].store(1);
+    }
+    chol_backsolve_band_kernel<<<1, 512, (size_t) n * sizeof(double), st>>>(Lmat, n, n, linv_ws, B.env, x);
+    BSFM_KERNEL_CHECK();
+    return BSFM_OK;
 }
 
 __global__ void __launch_bounds__(512) chol_backsolve_blocked_kernel(const double *A, int ld, int n, const double *Linv_all, double *x, double *ywork);

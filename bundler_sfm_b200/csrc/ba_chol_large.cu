@@ -675,8 +675,21 @@ static int set_smem_attr_once(int dev)
 
 // Same contract as chol_solve (ba_chol.cu): symmetric A (both triangles) + right-hand side in row n; Lmat (n+1) x n;
 // linv_ws ceil(n/32) * 1024 doubles; xinv_ws ceil(n/256) * 65536 doubles (L_pp^-T of every panel); x receives the solution.
-int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *xinv_ws, double *x, Scalars *sc)
+// band: a fitting envelope plan (ba_order.cu: chol_band_plan).  The system then takes the one-launch band factorisation and the
+// envelope-bounded back substitution instead of the panels below (entries of A outside the envelope are taken as zero).
+int chol_solve_large(cudaStream_t st, double *A, double *Lmat, int n, double *linv_ws, double *xinv_ws, double *x, Scalars *sc,
+                     const CholBand *band)
 {
+    if (band && band->env) {
+        g_prof.begin(0, st);
+        int rc = chol_band_factor(st, A, Lmat, n, linv_ws, *band, sc);
+        g_prof.end(st);
+        if (rc != BSFM_OK) return rc;
+        g_prof.begin(3, st);
+        rc = chol_band_backsolve(st, Lmat, n, linv_ws, *band, x);
+        g_prof.end(st);
+        return rc;
+    }
     const int ld = n, nrows = n + 1;
     int dev = 0;
     BSFM_CUDA_TRY(cudaGetDevice(&dev));

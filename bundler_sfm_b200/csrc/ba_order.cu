@@ -182,20 +182,115 @@ int camera_order(int m, int mcon, int cnp, const uint32_t *keys, int nblocks, st
     return 1;
 }
 
-int apply_camera_order(Problem &P, int cnp, cudaStream_t st, DeviceArena &D)
+// first nonzero column of every row of S in the camera order pos: row block q of camera position q starts at
+// cnp x min(position of q's neighbours and of q itself)
+static std::vector<int> band_first_cols(int m, int mcon, int cnp, const uint32_t *keys, int nblocks, const std::vector<int> &pos)
+{
+    const int nf = m - mcon;
+    std::vector<int> lo(pos);      // lo[v]: lowest position among camera v and its neighbours
+    for (int b = 0; b < nblocks; b++) {
+        const int j = (int) (keys[b] / (uint32_t) m), k = (int) (keys[b] % (uint32_t) m);
+        if (j < mcon || k < mcon) continue;
+        lo[j - mcon] = std::min(lo[j - mcon], pos[k - mcon]);
+        lo[k - mcon] = std::min(lo[k - mcon], pos[j - mcon]);
+    }
+    std::vector<int> first((size_t) nf * cnp);
+    for (int v = 0; v < nf; v++)
+        for (int r = 0; r < cnp; r++) first[(size_t) pos[v] * cnp + r] = lo[v] * cnp;
+    return first;
+}
+
+// The tiles with an update step, by interval colouring in order of first step (ties: ascending tile index): each takes the
+// lowest colour whose previous tile finished before it starts, so the colours used are the largest live set and every
+// colour's tiles follow each other in increasing step.  Colour c is slot c / workers of worker c % workers.
+void chol_band_plan(int n, const int *first_col, int max_workers, CholBandPlan &plan)
+{
+    plan = CholBandPlan();
+    const int nbk = (n + LNB - 1) / LNB;
+    plan.n = n; plan.nbk = nbk;
+    plan.env.assign(nbk + 1, 0);
+    for (int rb = 0; rb < nbk; rb++) {
+        int e = rb * LNB;
+        for (int i = rb * LNB; i < std::min(n, (rb + 1) * LNB); i++) e = std::min(e, std::max(0, std::min(first_col[i], i)));
+        plan.env[rb] = e / LNB;
+    }
+    plan.toff.assign(nbk + 2, 0);
+    for (int rb = 0; rb <= nbk; rb++) plan.toff[rb + 1] = plan.toff[rb] + (rb == nbk ? nbk : rb - plan.env[rb] + 1);
+    plan.ntile = plan.toff[nbk + 1];
+    struct Live { int kf, kl, rb, cb; };
+    std::vector<Live> live;
+    for (int rb = 0; rb <= nbk; rb++)
+        for (int cb = plan.env[rb]; cb < std::min(rb + 1, nbk); cb++) {
+            const int kf = std::max(plan.env[rb], plan.env[cb]), kl = (rb == cb) ? cb - 2 : cb - 1;
+            if (kf <= kl) live.push_back({kf, kl, rb, cb});
+        }
+    std::vector<int> starts(nbk + 1, 0), ends(nbk + 1, 0);
+    for (const Live &t : live) { starts[t.kf]++; ends[t.kl]++; }
+    for (int k = 0, cur = 0; k < nbk; k++) { cur += starts[k]; plan.max_live = std::max(plan.max_live, cur); cur -= ends[k]; }
+    plan.workers = std::max(1, std::min(max_workers, plan.max_live));
+    plan.fits = n > CHOL_BAND_MIN_N && n <= CHOL_BAND_MAX_N && max_workers >= 1 && plan.max_live <= 2 * plan.workers &&
+                (size_t) plan.ntile <= chol_band_capacity_tiles(n);
+    if (!plan.fits) return;      // a wide envelope is refused before the colouring, whose cost grows with its width
+    // intervals in order of start: the lowest free colour uses exactly max_live colours
+    std::stable_sort(live.begin(), live.end(), [](const Live &a, const Live &b) { return a.kf < b.kf; });
+    std::vector<int> colour_end, colour(live.size());      // last step of every colour's latest tile
+    for (size_t t = 0; t < live.size(); t++) {
+        int c = 0;
+        while (c < (int) colour_end.size() && colour_end[c] >= live[t].kf) c++;
+        if (c == (int) colour_end.size()) colour_end.push_back(0);
+        colour_end[c] = live[t].kl;
+        colour[t] = c;
+    }
+    const int W = plan.workers;
+    plan.sptr.assign(2 * W + 1, 0);
+    for (size_t t = 0; t < live.size(); t++) plan.sptr[2 * (colour[t] % W) + colour[t] / W + 1]++;
+    for (int s = 0; s < 2 * W; s++) plan.sptr[s + 1] += plan.sptr[s];
+    plan.sched.resize(live.size());
+    std::vector<int> fill(plan.sptr.begin(), plan.sptr.end() - 1);
+    for (size_t t = 0; t < live.size(); t++) plan.sched[fill[2 * (colour[t] % W) + colour[t] / W]++] = live[t].rb << 16 | live[t].cb;
+}
+
+int apply_camera_order(Problem &P, int cnp, cudaStream_t st, DeviceArena &D, CholBand &band)
 {
     static const bool on = []() { const char *e = getenv("BSFM_BA_CAMERA_ORDER"); return !(e && e[0] == '0'); }();
     P.cam_pos = nullptr;
-    if (!on || (int64_t) (P.m - P.mcon) * cnp <= CHOL_LARGE_MIN || P.nblocks <= 0) return BSFM_OK;
+    band = CholBand();
+    const int nf = P.m - P.mcon;
+    const int64_t nsys = (int64_t) nf * cnp;
+    if (nsys <= CHOL_LARGE_MIN || P.nblocks <= 0 || (!on && nsys <= CHOL_BAND_MIN_N)) return BSFM_OK;
     std::vector<uint32_t> keys(P.nblocks);
     BSFM_CUDA_TRY(cudaMemcpyAsync(keys.data(), P.blk_key, keys.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     BSFM_CUDA_TRY(cudaStreamSynchronize(st));
-    std::vector<int> pos;
+    std::vector<int> pos(nf);
+    for (int v = 0; v < nf; v++) pos[v] = v;
     int64_t scores[2];
-    if (!camera_order(P.m, P.mcon, cnp, keys.data(), P.nblocks, pos, scores)) return BSFM_OK;
-    int *d_pos;
-    TRY(D.upload(&d_pos, pos.data(), pos.size()));      // pageable source: the copy is staged before it returns
-    P.cam_pos = d_pos;
+    const bool rcm = on && camera_order(P.m, P.mcon, cnp, keys.data(), P.nblocks, pos, scores);
+    if (rcm) {
+        int *d_pos;
+        TRY(D.upload(&d_pos, pos.data(), pos.size()));      // pageable source: the copy is staged before it returns
+        P.cam_pos = d_pos;
+    }
+    // the envelope of S in the order it is factored in; its plan, when it fits, replaces the panel path
+    if (nsys <= CHOL_BAND_MIN_N) return BSFM_OK;
+    int dev = 0, sms = 0;
+    BSFM_CUDA_TRY(cudaGetDevice(&dev));
+    BSFM_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const std::vector<int> first = band_first_cols(P.m, P.mcon, cnp, keys.data(), P.nblocks, pos);
+    CholBandPlan plan;
+    chol_band_plan(nf * cnp, first.data(), sms - 1, plan);
+    if (!plan.fits) return BSFM_OK;
+    return upload_band_plan(plan, D, band);
+}
+
+int upload_band_plan(const CholBandPlan &plan, DeviceArena &D, CholBand &band)
+{
+    int *env, *toff, *sptr, *sched;
+    TRY(D.upload(&env, plan.env.data(), plan.env.size()));
+    TRY(D.upload(&toff, plan.toff.data(), plan.toff.size()));
+    TRY(D.upload(&sptr, plan.sptr.data(), plan.sptr.size()));
+    TRY(D.upload(&sched, plan.sched.data(), plan.sched.size()));
+    band.env = env; band.toff = toff; band.sptr = sptr; band.sched = sched;
+    band.ntile = plan.ntile; band.workers = plan.workers;
     return BSFM_OK;
 }
 
@@ -218,4 +313,18 @@ extern "C" int bsfm_ba_camera_order(int m, int mcon, int cnp, const uint32_t *bl
     const int rcm = ba::camera_order(m, mcon, cnp, blk_key, nblocks, pos, scores);
     std::copy(pos.begin(), pos.end(), cam_pos);
     return rcm;
+}
+
+extern "C" int bsfm_ba_chol_band_plan(int n, const int32_t *first_col, int workers, int32_t *env, int64_t out[3])
+{
+    using namespace bsfm;
+    clear_error();
+    if (n <= 0 || n > (1 << 20) || !first_col || workers < 1 || !out) { set_error("bsfm_ba_chol_band_plan: bad arguments"); return BSFM_ERR_ARG; }
+    for (int i = 0; i < n; i++)
+        if (first_col[i] < 0 || first_col[i] > i) { set_error("bsfm_ba_chol_band_plan: first_col[%d] = %d is not in [0, %d]", i, first_col[i], i); return BSFM_ERR_ARG; }
+    ba::CholBandPlan plan;
+    ba::chol_band_plan(n, first_col, workers, plan);
+    if (env) std::copy(plan.env.begin(), plan.env.end(), env);
+    out[0] = plan.ntile; out[1] = plan.max_live; out[2] = plan.fits ? plan.workers : 0;
+    return plan.fits ? 1 : 0;
 }

@@ -6,6 +6,7 @@
 #include <vector>
 #include "common.h"
 #include "ba_kernels.cuh"
+#include "ba_chol_large.cuh"
 
 #define TRY(expr) do { int rc__ = (expr); if (rc__ != BSFM_OK) return rc__; } while (0)
 
@@ -90,8 +91,12 @@ int build_schur_structure(Problem &P, cudaStream_t st, DeviceArena &D);
 // RCM is taken, 0 when the natural order is kept (then pos is the identity).
 int camera_order(int m, int mcon, int cnp, const uint32_t *keys, int nblocks, std::vector<int> &pos, int64_t scores[2]);
 // Applies it to P (sets P.cam_pos) when the system takes the large Cholesky path and RCM wins; BSFM_BA_CAMERA_ORDER=0 keeps
-// the natural order.  Reads P.blk_key back to the host (one synchronisation of st).
-int apply_camera_order(Problem &P, int cnp, cudaStream_t st, DeviceArena &D);
+// the natural order.  Then plans the band factorisation of S in that order (chol_band_plan) and uploads the plan into `band`
+// when it fits (otherwise band.env stays null and the panel path runs).  Reads P.blk_key back to the host (one
+// synchronisation of st).
+int apply_camera_order(Problem &P, int cnp, cudaStream_t st, DeviceArena &D, CholBand &band);
+// a fitting band plan -> its device copy, in D
+int upload_band_plan(const CholBandPlan &plan, DeviceArena &D, CholBand &band);
 
 }  // namespace ba
 }  // namespace bsfm

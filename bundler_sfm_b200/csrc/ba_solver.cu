@@ -105,6 +105,7 @@ struct Solve {
     PhaseTimer PT;
     HostMarks HM;
     Problem P{};
+    CholBand band;            // envelope plan of S in its factorisation order (apply_camera_order), or none
     int nvis = 0, nobs = 0, useg = 0, red_blocks_obs = 0, red_blocks_var = 0;
     double *d_p, *d_pdp, *d_e, *d_enew, *d_camR_a, *d_camR_b, *d_Lmat, *d_linv, *d_da, *d_mu;
     double *const h_mu;
@@ -333,7 +334,7 @@ int Solve::controller(int itmax, int verbose, const double opts[6], bool any_con
             TRY(schur(!s_dense));   // camera pairs without a common point keep S_jk = 0
             PT.end();
             PT.begin(3);
-            TRY(chol_solve(st, P.S, d_Lmat, Sdim, d_linv, d_da, P.sc));
+            TRY(chol_solve(st, P.S, d_Lmat, Sdim, d_linv, d_da, P.sc, &band));
             PT.end();
             PT.begin(4);
             BA_LAUNCH(backsub_kernel, (std::max(n, m * cnp) + 127) / 128, 128, P, d_da);
@@ -482,7 +483,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     S.PT.begin(0);
     TRY(S.visibility(vis, x));
     TRY(build_schur_structure(S.P, st, S.D));
-    if (!mot) TRY(apply_camera_order(S.P, cnp, st, S.D));      // large systems: S in the order that skips most of the factorisation
+    if (!mot) TRY(apply_camera_order(S.P, cnp, st, S.D, S.band));      // large systems: S in the order that skips most of the factorisation
     S.HM.mark("Schur structure + camera order");
     TRY(S.upload(model, init_params, fisheye != 0, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints));
     S.PT.end();
@@ -588,15 +589,29 @@ struct CholOutputs {
     double *L, *linv, *xinv;
     int *fail_code;
 };
-static int axb_chol_impl(const double *A, const double *B, double *x, int m, int reps, float *ms_out, const CholOutputs *out = nullptr)
+// first_col (bsfm_sba_Axb_Chol_factor_env): the caller's row envelope; a large system whose plan fits takes the band path
+static int axb_chol_impl(const double *A, const double *B, double *x, int m, int reps, float *ms_out, const CholOutputs *out = nullptr,
+                         const int32_t *first_col = nullptr)
 {
     clear_error();
     TRY(require_device());
     if (!A || !B || !x || m <= 0 || reps < 1) { set_error("bsfm_sba_Axb_Chol: bad arguments"); return BSFM_ERR_ARG; }
+    if (first_col)
+        for (int i = 0; i < m; i++)
+            if (first_col[i] < 0 || first_col[i] > i) { set_error("bsfm_sba_Axb_Chol_factor_env: first_col[%d] = %d is not in [0, %d]", i, first_col[i], i); return BSFM_ERR_ARG; }
     cudaStream_t st;
     BSFM_CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{st};
     DeviceArena D(st);   // after the guard: the arena waits for the stream and returns its blocks before the stream goes
+    CholBand band;
+    if (first_col && m > CHOL_LARGE_MIN) {
+        int dev = 0, sms = 0;
+        BSFM_CUDA_TRY(cudaGetDevice(&dev));
+        BSFM_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        CholBandPlan plan;
+        chol_band_plan(m, first_col, sms - 1, plan);
+        if (plan.fits) TRY(upload_band_plan(plan, D, band));
+    }
     double *d_src, *d_A, *d_L, *d_linv, *d_x; Scalars *d_sc;
     const size_t mm = (size_t) m * m;
     TRY(D.alloc(&d_src, mm + m)); TRY(D.alloc(&d_A, mm + m)); TRY(D.alloc(&d_L, mm + m));
@@ -613,7 +628,7 @@ static int axb_chol_impl(const double *A, const double *B, double *x, int m, int
     for (int r = 0; r < reps && rc == BSFM_OK; r++) {
         cudaMemcpyAsync(d_A, d_src, (mm + m) * sizeof(double), cudaMemcpyDeviceToDevice, st);
         cudaEventRecord(e0, st);
-        rc = chol_solve(st, d_A, d_L, m, d_linv, d_x, d_sc);
+        rc = chol_solve(st, d_A, d_L, m, d_linv, d_x, d_sc, &band);
         cudaEventRecord(e1, st);
         if (cudaStreamSynchronize(st) != cudaSuccess) { set_error("bsfm_sba_Axb_Chol: %s", cudaGetErrorString(cudaGetLastError())); rc = BSFM_ERR_CUDA; }
         float t = 0.f; cudaEventElapsedTime(&t, e0, e1); total += t;
@@ -640,6 +655,13 @@ extern "C" int bsfm_sba_Axb_Chol_factor(const double *A, const double *B, double
 {
     const CholOutputs out = {L, linv, xinv, fail_code};
     return axb_chol_impl(A, B, x, m, 1, nullptr, &out);
+}
+extern "C" int bsfm_sba_Axb_Chol_factor_env(const double *A, const double *B, double *x, int m, const int32_t *first_col, double *L, double *linv,
+                                            double *xinv, int *fail_code)
+{
+    if (!first_col) { clear_error(); set_error("bsfm_sba_Axb_Chol_factor_env: first_col is NULL"); return BSFM_ERR_ARG; }
+    const CholOutputs out = {L, linv, xinv, fail_code};
+    return axb_chol_impl(A, B, x, m, 1, nullptr, &out, first_col);
 }
 extern "C" int bsfm_sba_Axb_Chol(const double *A, const double *B, double *x, int m, int iscolmaj)
 {

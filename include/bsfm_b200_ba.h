@@ -280,6 +280,18 @@ int bsfm_sba_Axb_Chol_timed(const double *A, const double *B, double *x, int m, 
  *              dataflow kernel (csrc/ba_chol_dataflow.cu) that never arrived.  Any nonzero value returns 0.       */
 int bsfm_sba_Axb_Chol_factor(const double *A, const double *B, double *x, int m, double *L, double *linv, double *xinv,
                              int *fail_code);
+/* Test entry: bsfm_sba_Axb_Chol_factor on a matrix with the caller's row envelope: first_col[i] (0 <= first_col[i] <= i)
+ * is the first nonzero column of row i, and entries of A left of it are taken as zero.  For m > 4096 whose band plan fits
+ * (bsfm_ba_chol_band_plan with the device's SM count - 1 workers) the one-launch band factorisation runs; L is then written
+ * on the envelope's 32 x 32 tiles only, and xinv is not written.  Otherwise the same solve as bsfm_sba_Axb_Chol_factor.   */
+int bsfm_sba_Axb_Chol_factor_env(const double *A, const double *B, double *x, int m, const int32_t *first_col, double *L,
+                                 double *linv, double *xinv, int *fail_code);
+/* The band plan of an n x n system with row envelope first_col (host only): env (may be NULL; ceil(n/32) + 1 entries)
+ * receives the first tile column of every 32-row block (the right-hand-side row last, 0); out[0] = tiles of the envelope,
+ * right-hand-side row included, out[1] = the largest number of tiles taking updates at one step, out[2] = worker CTAs the
+ * schedule uses (0 when it does not fit).  Returns 1 when 4096 < n <= 24576 and the plan fits `workers` CTAs of two tile
+ * slots each and the solver's workspace, 0 when not, < 0 on bad arguments.  Smaller systems keep the panel path.                                                                 */
+int bsfm_ba_chol_band_plan(int n, const int32_t *first_col, int workers, int32_t *env, int64_t out[3]);
 
 /* Per-kernel-class device timing of the large-system Cholesky (systems > 1536 unknowns), for roofline reporting:
  * bsfm_ba_chol_profile(1) resets the counters of the calling thread and records CUDA events around every launch of
@@ -287,7 +299,8 @@ int bsfm_sba_Axb_Chol_factor(const double *A, const double *B, double *x, int m,
  * [0] diagonal-block factorisation  [1] panel solve  [2] trailing update  [3] back substitution,
  * and the fp64 FLOPs of the trailing update (2 per multiply-add of the lower triangle).  Call it after the solves
  * have completed.  [0] includes the diagonal blocks the look-ahead factors on its side stream, next to the trailing update
- * (their time overlaps [2]).                                                                                        */
+ * (their time overlaps [2]).  On the band path (a banded system whose plan fits) the one factorisation launch counts in
+ * [0], its back substitution in [3], and [1], [2] and the FLOPs stay 0.                                              */
 int bsfm_ba_chol_profile(int enable);
 int bsfm_ba_chol_profile_read(float ms[4], int launches[4], double *fp64_flops);
 

@@ -4,6 +4,9 @@ per process): `warmup` untimed solves, then `rounds` solves with the per-phase e
 events of the large Cholesky (bsfm_ba_chol_profile: diagonal blocks, look-ahead side stream included; panel solves; trailing
 updates; back substitution).  Reports per solve: phases, kernel classes, launches, executed trailing-update FLOPs, LM
 iterations, stop reason and nlss, and the host time of the order itself (bsfm_ba_camera_order on the scene's Schur blocks).
+With the order, config 3's system is banded and takes the one-launch band factorisation (ba_chol_dataflow.cu: its launch
+counts as "diag_block", its back substitution as "back_substitution", no panel solve or update runs; "path" says which);
+without it the envelope is too wide and the panel path runs, so the two children show the two paths side by side.
 Needs the GPU; prints the GPU name and power limit of the run (nvidia-smi, read-only).
 
 usage: python scripts/bench_camera_order.py [--rounds 3] [--warmup 1]"""
@@ -83,6 +86,7 @@ def child(rounds, warmup):
     med = np.median(np.asarray(classes), axis=0)
     res = {
         "camera_order": os.environ.get("BSFM_BA_CAMERA_ORDER", "1"),
+        "path": "band" if launches[-1][1] == 0 and launches[-1][2] == 0 else "panels",
         "iterations": int(infos[-1][5]), "stop": int(infos[-1][6]), "nlss": int(infos[-1][9]),
         "phase_ms_median": {k: float(np.median([p[k] for p in phases])) for k in phases[0] if k.endswith("_ms")},
         "cholesky_class_ms_median": dict(zip(names, map(float, med))),
