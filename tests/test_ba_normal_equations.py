@@ -519,14 +519,20 @@ def analytic_step_ratios(name):
     assert rc == 1 and int(info[7]) == 2 and int(info[9]) == 1, (name, rc, info)
     A, B = rs.jacobian_exact(P, p)
     e = P.x - rs.evaluate(P, p)
-    blk = rs.normal_blocks(P, p, A, B, e)
+    return damped_step_ratios(P, p, p1, info, rs.normal_blocks(P, p, A, B, e), e, name)
+
+
+def damped_step_ratios(P, p, p1, info, blk, e, name=""):
+    """analytic_step_ratios' checks of p1 = the GPU's p after one accepted iteration from p, given the restatement's
+    normal-equation blocks blk of the exact Jacobian and the residual e at p"""
     mu = 1e-3 * rs.max_diag(P, blk)
     S, E, Vinv = rs.schur(P, blk, mu)
     dp = rs.solve_reduced(P, blk, S, E, Vinv)
     p_eL2 = float(np.sum(e * e)) + rs.penalty(P, p)
     ok, pdp_eL2, dL = _accepted(P, p, dp, mu, blk, p_eL2)
     assert ok, name
-    t = (np.bincount(P.cj).max() + 100) * u * np.linalg.cond(S)
+    lam = np.linalg.eigvalsh(S)                       # S is SPD: cond_2(S) = lam_max / lam_min, without an SVD
+    t = (np.bincount(P.cj).max() + 100) * u * (lam[-1] / lam[0])
     da, db = dp[:P.ncp], dp[P.ncp:].reshape(P.n, 3)
     gda, gdb = (p1 - p)[:P.ncp], (p1 - p)[P.ncp:].reshape(P.n, 3)
     sda = float(np.max(np.abs(da)))

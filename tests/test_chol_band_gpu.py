@@ -46,9 +46,15 @@ def factorise_env(A, b, first):
     return rc, fail.value, x, L, linv, list(launches)
 
 
+def workers():
+    """worker CTAs of the band plan on this device: SM count - 1 (131 on an H100 SXM, 113 on an H100 PCIe)"""
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count - 1
+
+
 def widest_fitting(n):
     w = 1
-    while B.band_plan(B.tile_band_first(n, w + 1), n, 131)[0]:
+    while B.band_plan(B.tile_band_first(n, w + 1), n, workers())[0]:
         w += 1
     return w
 
@@ -66,7 +72,7 @@ CASES = {
 
 def _check_band_exact(n, first, seed):
     L0, A, x0, b = B.envelope_system(first, seed=seed)
-    fits = B.band_plan(first, n, 131)[0]
+    fits = B.band_plan(first, n, workers())[0]
     assert fits
     rc, fail, x, L, linv, launches = factorise_env(A, b, first)
     assert (rc, fail) == (1, 0), (rc, fail)
@@ -127,7 +133,7 @@ def test_precision_bound_on_random_banded_systems():
 def test_mid_size_banded_systems_keep_the_panel_path(n):
     """systems of at most 4096 unknowns keep the panel path whatever their envelope, with the exact answer"""
     first = B.tile_band_first(n, 2)
-    assert not B.band_plan(first, n, 131)[0]
+    assert not B.band_plan(first, n, workers())[0]
     L0, A, x0, b = B.envelope_system(first, seed=5)
     rc, fail, x, L, linv, launches = factorise_env(A, b, first)
     assert (rc, fail) == (1, 0)
@@ -139,7 +145,7 @@ def test_wide_envelope_takes_the_panel_path():
     """a plan that does not fit (every row reaches column 0) runs the panel path on the same entry, with the same results"""
     n = 4500
     first = np.zeros(n, np.int32)
-    assert not B.band_plan(first, n, 131)[0]
+    assert not B.band_plan(first, n, workers())[0]
     L0, A, x0, b = B.envelope_system(B.tile_band_first(n, 4), seed=3)
     rc, fail, x, L, linv, launches = factorise_env(A, b, first)
     assert (rc, fail) == (1, 0)
