@@ -377,3 +377,53 @@ def reprojection_outliers(scene, estimate_distortion=1, min_thresh=8.0, max_thre
     check(rc, name)
     k = min(rc, cap)
     return {"dist": dist, "stats": stats, "outliers": out_idx[:k].copy(), "errors": out_err[:k].copy(), "global_mean": gm.value, "count": rc}
+
+
+class SfmRound(ctypes.Structure):
+    """== bsfm_sfm_round_t (include/bsfm_b200_ba.h)"""
+    _fields_ = [("num_pts", ctypes.c_int32), ("nvis", ctypes.c_int32), ("num_outliers", ctypes.c_int32), ("removed", ctypes.c_int32),
+                ("info", ctypes.c_double * 10), ("global_mean", ctypes.c_double),
+                ("h2d_bytes", ctypes.c_int64), ("h2d_largest", ctypes.c_int64)]
+
+
+def run_sfm_outlier_loop(scene, est_focal_length=1, undistort=1, explicit_camera_centers=1, ncons=0, eps2=1e-12,
+                         use_constraints=0, constrained=None, constraints=None, weights=None,
+                         use_point_constraints=0, points_constraints=None, point_constraint_weight=0.0, fix_points=0,
+                         known=None, K_known=None, k_known=None, fisheye=None, fisheye_params=None, optimize_for_fisheye=0,
+                         remove_outliers=1, min_outliers=40, min_points=20, min_thresh=8.0, max_thresh=16.0, rounds_cap=64,
+                         pt_round=True):
+    """bsfm_run_sfm_outlier_loop: the solve / outlier-removal loop of BundlerApp::RunSFM_SBA (src/Bundle.cpp:568-919) on a
+    CRS scene (synth.crs_scene), with the scene on the GPU between rounds.  Camera and constraint keywords are those of
+    call_run_sfm; min_outliers / min_points / min_thresh / max_thresh default to Bundler's.  Returns the refined R, c, f, k,
+    pts (by original point index), pt_round, pt_error, cam_stats of the last round, rounds (a list of dicts, at most
+    rounds_cap of them), count (rounds run) and mean_error.  pt_round=False passes a null pt_round (refused)."""
+    fn = load_library().bsfm_run_sfm_outlier_loop
+    c = ctypes
+    fn.argtypes = [c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_int,
+                   c.c_void_p, c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_double, c.c_int, c.c_int, c.c_double,
+                   c.c_int, c.c_int, c.c_int, c.c_double, c.c_double, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_int, c.c_void_p]
+    fn.restype = c.c_int
+    assert "vis_ptr" in scene, "run_sfm_outlier_loop takes a CRS scene (synth.crs_scene)"
+    n, m, vis_args, _keep = _visibility_args(scene)
+    proj = np.ascontiguousarray(scene["projections"], dtype=np.float64)
+    cams = make_cameras(scene["R"], scene["c"], scene["f"], scene["k"], constrained, constraints, weights, known, K_known, k_known,
+                        fisheye, fisheye_params)
+    pts = np.ascontiguousarray(scene["pts"], dtype=np.float64).copy()
+    pc = np.ascontiguousarray(points_constraints, dtype=np.float64) if use_point_constraints else None
+    rnd = np.full(n, -9, np.int32)
+    err = np.zeros(n)
+    stats = np.zeros((m, 5))
+    rounds = (SfmRound * max(rounds_cap, 1))()
+    mean = c.c_double()
+    rc = fn(n, m, ncons, *vis_args, proj.ctypes.data, est_focal_length, 0, undistort, explicit_camera_centers,
+            c.addressof(cams), pts.ctypes.data, use_constraints, use_point_constraints, pc.ctypes.data if pc is not None else None,
+            float(point_constraint_weight), int(fix_points), int(optimize_for_fisheye), float(eps2),
+            int(remove_outliers), int(min_outliers), int(min_points), float(min_thresh), float(max_thresh),
+            rnd.ctypes.data if pt_round else None, err.ctypes.data, stats.ctypes.data, c.addressof(rounds), int(rounds_cap), c.byref(mean))
+    check(rc, "bsfm_run_sfm_outlier_loop")
+    R, cc, f, k = cameras_to_arrays(cams)
+    out_rounds = [{"num_pts": r.num_pts, "nvis": r.nvis, "num_outliers": r.num_outliers, "removed": r.removed,
+                   "info": np.array(list(r.info)), "global_mean": r.global_mean, "h2d_bytes": r.h2d_bytes, "h2d_largest": r.h2d_largest}
+                  for r in rounds[:min(rc, rounds_cap)]]
+    return {"count": rc, "R": R, "c": cc, "f": f, "k": k, "pts": pts, "pt_round": rnd, "pt_error": err, "cam_stats": stats,
+            "rounds": out_rounds, "mean_error": mean.value}

@@ -19,14 +19,11 @@
 
 #include "common.h"
 #include "ba_kernels.cuh"
-#include "ba_setup.h"
+#include "ba_loop.h"
 #include "../../include/bsfm_b200_ba.h"
 
 namespace bsfm {
 namespace ba {
-
-struct CamCompact { double R[9], t[3], f, k0, k1; };
-struct Rot3 { double R[9]; };
 
 // ImageData::DistortPoint (ImageData.cpp:1129-1169) of a fisheye camera, in the reference's operation order: the ray
 // (x, y, -f_focal) is rotated by `Rs`; when its z is not positive the point is left as it is (the reference returns
@@ -135,7 +132,74 @@ __global__ void outlier_err_kernel(int nvis, const int *obs_cam, const int *obs_
 using namespace bsfm;
 using namespace bsfm::ba;
 
-// the outlier pass on either visibility source (bsfm_reprojection_outliers, bsfm_reprojection_outliers_crs)
+// camera tables of a pass (what the loop reads: R, t = centre, f, k; calibrated and fisheye side tables when present)
+int bsfm::ba::upload_outlier_cams(const bsfm_camera_params_t *cams, int m, int optimize_for_fisheye, DeviceArena &D, OutlierCams &T)
+{
+    std::vector<CamCompact> hc(m);
+    bool any_known = false;
+    for (int j = 0; j < m; j++) {
+        memcpy(hc[j].R, cams[j].R, sizeof hc[j].R); memcpy(hc[j].t, cams[j].t, sizeof hc[j].t);
+        hc[j].f = cams[j].f; hc[j].k0 = cams[j].k[0]; hc[j].k1 = cams[j].k[1];
+        any_known = any_known || cams[j].known_intrinsics;
+    }
+    TRY(D.upload(&T.cams, hc.data(), (size_t) m));
+    if (any_known) {     // calibrated cameras (sfm.c:339-357): side table, only when there is one
+        std::vector<CamIntrinsics> hi(m);
+        for (int j = 0; j < m; j++) hi[j] = cam_intrinsics(cams[j]);
+        TRY(D.upload(&T.intr, hi.data(), (size_t) m));
+    }
+    if (optimize_for_fisheye) {   // fisheye cameras: side table, only when the call asks for their mapping
+        std::vector<CamFisheye> hf(m);
+        for (int j = 0; j < m; j++) hf[j] = cam_fisheye(cams[j]);
+        TRY(D.upload(&T.fe, hf.data(), (size_t) m));
+        // GetRotationFromSpherical(-pi/2, pi/2) (BundleUtil.cpp:70-94), with the host libm like the reference: the identity
+        // up to +-6.1e-17 terms, which change the last bits of the result
+        const double theta = -0.5 * M_PI, phi = 0.5 * M_PI;
+        const double v[3] = {cos(theta) * sin(phi), cos(phi), sin(theta) * sin(phi)};
+        const double phi_up = phi - 0.5 * M_PI, theta_up = theta;
+        const double up[3] = {cos(theta_up) * sin(phi_up), cos(phi_up), sin(theta_up) * sin(phi_up)};
+        const double x_axis[3] = {v[1] * up[2] - v[2] * up[1], v[2] * up[0] - v[0] * up[2], v[0] * up[1] - v[1] * up[0]};
+        for (int q = 0; q < 3; q++) { T.Rs.R[q] = x_axis[q]; T.Rs.R[3 + q] = up[q]; T.Rs.R[6 + q] = v[q]; }
+    }
+    return BSFM_OK;
+}
+
+int bsfm::ba::outliers_core(const Visibility &vis, int n, int m, const OutlierCams &T, const double *d_pts, const double *d_proj,
+                            int estimate_distortion, double min_thresh, double max_thresh, const char *d_prot, cudaStream_t st,
+                            DeviceArena &D, OutlierPass &out)
+{
+    const int nvis = vis.nvis;
+    double *d_dist_cam, *d_dist_sorted;
+    TRY(D.alloc(&out.dist, (size_t) nvis)); TRY(D.alloc(&d_dist_cam, (size_t) nvis)); TRY(D.alloc(&d_dist_sorted, (size_t) nvis));
+    TRY(D.alloc(&out.stats, (size_t) m * 5)); TRY(D.alloc(&out.err, (size_t) n));
+    TRY(D.alloc(&out.first_cam, (size_t) n));
+    const int gb = (nvis + 255) / 256;
+    const int ud = estimate_distortion ? 1 : 0;
+    if (T.fe) {
+        if (T.intr) outlier_dist_kernel<true, true><<<gb, 256, 0, st>>>(nvis, vis.obs_cam, vis.obs_pt, T.cams, T.intr, T.fe, T.Rs, d_pts, d_proj, ud, out.dist);
+        else outlier_dist_kernel<false, true><<<gb, 256, 0, st>>>(nvis, vis.obs_cam, vis.obs_pt, T.cams, nullptr, T.fe, T.Rs, d_pts, d_proj, ud, out.dist);
+    } else {
+        if (T.intr) outlier_dist_kernel<true, false><<<gb, 256, 0, st>>>(nvis, vis.obs_cam, vis.obs_pt, T.cams, T.intr, nullptr, T.Rs, d_pts, d_proj, ud, out.dist);
+        else outlier_dist_kernel<false, false><<<gb, 256, 0, st>>>(nvis, vis.obs_cam, vis.obs_pt, T.cams, nullptr, nullptr, T.Rs, d_pts, d_proj, ud, out.dist);
+    }
+    BSFM_KERNEL_CHECK();
+
+    // per-camera sorted distances, in the camera-major view (ascending point order within each camera)
+    outlier_gather_kernel<<<gb, 256, 0, st>>>(nvis, vis.cam_obs, out.dist, d_dist_cam);
+    BSFM_KERNEL_CHECK();
+    TRY(D.cub(3, [&](void *t, size_t &b) { return cub::DeviceSegmentedSort::SortKeys(t, b, d_dist_cam, d_dist_sorted, nvis, m, vis.cam_ptr, vis.cam_ptr + 1, st); }));
+    outlier_cam_stats_kernel<<<(m * 32 + 255) / 256, 256, 0, st>>>(m, vis.cam_ptr, d_dist_cam, d_dist_sorted, min_thresh, max_thresh, out.stats);
+    BSFM_KERNEL_CHECK();
+    BSFM_CUDA_TRY(cudaMemsetAsync(out.first_cam, 0x7f, (size_t) n * sizeof(int), st));      // 0x7f7f7f7f: larger than any camera index
+    outlier_flag_kernel<<<gb, 256, 0, st>>>(nvis, vis.obs_cam, vis.obs_pt, out.dist, out.stats, d_prot, out.first_cam);
+    BSFM_KERNEL_CHECK();
+    outlier_err_kernel<<<gb, 256, 0, st>>>(nvis, vis.obs_cam, vis.obs_pt, out.dist, out.first_cam, out.err);
+    BSFM_KERNEL_CHECK();
+    return BSFM_OK;
+}
+
+// the outlier pass on either visibility source (bsfm_reprojection_outliers, bsfm_reprojection_outliers_crs): uploads,
+// outliers_core, downloads and the ordering of the list
 static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src, const double *projections,
                          const bsfm_camera_params_t *cams, const bsfm_v3_t *pts, int estimate_distortion, int fisheye_entry,
                          int optimize_for_fisheye, double min_proj_error_threshold, double max_proj_error_threshold,
@@ -149,11 +213,8 @@ static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src,
         set_error("bsfm_reprojection_outliers: bad arguments");
         return BSFM_ERR_ARG;
     }
-    bool any_known = false;
-    for (int j = 0; j < m; j++) {
+    for (int j = 0; j < m; j++)
         if (cams[j].fisheye && !fisheye_entry) { set_error("bsfm_reprojection_outliers: fisheye cameras are outside this entry; bsfm_reprojection_outliers_fe takes them"); return BSFM_ERR_UNSUPPORTED; }
-        any_known = any_known || cams[j].known_intrinsics;
-    }
 
     // the legacy default stream, as every copy below: callers may pass device pointers written on it
     DeviceArena D(0);
@@ -161,67 +222,18 @@ static int outliers_impl(int num_pts, int num_cameras, const VisSource &vis_src,
     TRY(build_visibility(vis_src, n, m, 0, D, vis));
     const int nvis = vis.nvis;
     if (nvis <= 0) { set_error("bsfm_reprojection_outliers: empty visibility mask"); return BSFM_ERR_ARG; }
-    int *d_obs_cam = vis.obs_cam, *d_obs_pt = vis.obs_pt, *d_cam_obs = vis.cam_obs, *d_cam_ptr = vis.cam_ptr;
 
-    // cameras (what the loop reads: R, t = centre, f, k), points, measurements
-    std::vector<CamCompact> hc(m);
-    for (int j = 0; j < m; j++) {
-        memcpy(hc[j].R, cams[j].R, sizeof hc[j].R); memcpy(hc[j].t, cams[j].t, sizeof hc[j].t);
-        hc[j].f = cams[j].f; hc[j].k0 = cams[j].k[0]; hc[j].k1 = cams[j].k[1];
-    }
-    CamCompact *d_cams; double *d_pts, *d_proj, *d_dist, *d_dist_cam, *d_dist_sorted, *d_stats, *d_err;
+    OutlierCams T;
+    TRY(upload_outlier_cams(cams, m, optimize_for_fisheye, D, T));
+    double *d_pts, *d_proj;
     char *d_prot = nullptr;
-    int *d_first;
-    TRY(D.alloc(&d_dist, (size_t) nvis)); TRY(D.alloc(&d_dist_cam, (size_t) nvis)); TRY(D.alloc(&d_dist_sorted, (size_t) nvis));
-    TRY(D.alloc(&d_stats, (size_t) m * 5)); TRY(D.alloc(&d_err, (size_t) n));
-    TRY(D.alloc(&d_first, (size_t) n));
-    TRY(D.upload(&d_cams, hc.data(), (size_t) m));
-    CamIntrinsics *d_intr = nullptr;     // calibrated cameras (sfm.c:339-357): side table, only when there is one
-    if (any_known) {
-        std::vector<CamIntrinsics> hi(m);
-        for (int j = 0; j < m; j++) hi[j] = cam_intrinsics(cams[j]);
-        TRY(D.upload(&d_intr, hi.data(), (size_t) m));
-    }
-    CamFisheye *d_fe = nullptr;         // fisheye cameras: side table, only when the call asks for their mapping
-    Rot3 Rs = {};
-    if (optimize_for_fisheye) {
-        std::vector<CamFisheye> hf(m);
-        for (int j = 0; j < m; j++) hf[j] = cam_fisheye(cams[j]);
-        TRY(D.upload(&d_fe, hf.data(), (size_t) m));
-        // GetRotationFromSpherical(-pi/2, pi/2) (BundleUtil.cpp:70-94), with the host libm like the reference: the identity
-        // up to +-6.1e-17 terms, which change the last bits of the result
-        const double theta = -0.5 * M_PI, phi = 0.5 * M_PI;
-        const double v[3] = {cos(theta) * sin(phi), cos(phi), sin(theta) * sin(phi)};
-        const double phi_up = phi - 0.5 * M_PI, theta_up = theta;
-        const double up[3] = {cos(theta_up) * sin(phi_up), cos(phi_up), sin(theta_up) * sin(phi_up)};
-        const double x_axis[3] = {v[1] * up[2] - v[2] * up[1], v[2] * up[0] - v[0] * up[2], v[0] * up[1] - v[1] * up[0]};
-        for (int q = 0; q < 3; q++) { Rs.R[q] = x_axis[q]; Rs.R[3 + q] = up[q]; Rs.R[6 + q] = v[q]; }
-    }
     TRY(D.upload(&d_pts, pts, (size_t) n * 3));
     TRY(D.upload(&d_proj, projections, (size_t) nvis * 2));
     if (pt_protected) TRY(D.upload(&d_prot, pt_protected, (size_t) n));
-    const int gb = (nvis + 255) / 256;
-    const int ud = estimate_distortion ? 1 : 0;
-    if (d_fe) {
-        if (d_intr) outlier_dist_kernel<true, true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, d_fe, Rs, d_pts, d_proj, ud, d_dist);
-        else outlier_dist_kernel<false, true><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, d_fe, Rs, d_pts, d_proj, ud, d_dist);
-    } else {
-        if (d_intr) outlier_dist_kernel<true, false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, d_intr, nullptr, Rs, d_pts, d_proj, ud, d_dist);
-        else outlier_dist_kernel<false, false><<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_cams, nullptr, nullptr, Rs, d_pts, d_proj, ud, d_dist);
-    }
-    BSFM_KERNEL_CHECK();
-
-    // per-camera sorted distances, in the camera-major view (ascending point order within each camera)
-    outlier_gather_kernel<<<gb, 256>>>(nvis, d_cam_obs, d_dist, d_dist_cam);
-    BSFM_KERNEL_CHECK();
-    TRY(D.cub(3, [&](void *t, size_t &b) { return cub::DeviceSegmentedSort::SortKeys(t, b, d_dist_cam, d_dist_sorted, nvis, m, d_cam_ptr, d_cam_ptr + 1); }));
-    outlier_cam_stats_kernel<<<(m * 32 + 255) / 256, 256>>>(m, d_cam_ptr, d_dist_cam, d_dist_sorted, min_proj_error_threshold, max_proj_error_threshold, d_stats);
-    BSFM_KERNEL_CHECK();
-    BSFM_CUDA_TRY(cudaMemset(d_first, 0x7f, (size_t) n * sizeof(int)));      // 0x7f7f7f7f: larger than any camera index
-    outlier_flag_kernel<<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_dist, d_stats, d_prot, d_first);
-    BSFM_KERNEL_CHECK();
-    outlier_err_kernel<<<gb, 256>>>(nvis, d_obs_cam, d_obs_pt, d_dist, d_first, d_err);
-    BSFM_KERNEL_CHECK();
+    OutlierPass pass;
+    TRY(outliers_core(vis, n, m, T, d_pts, d_proj, estimate_distortion, min_proj_error_threshold, max_proj_error_threshold, d_prot, 0, D, pass));
+    double *d_dist = pass.dist, *d_stats = pass.stats, *d_err = pass.err;
+    int *d_first = pass.first_cam;
 
     // results
     std::vector<double> stats((size_t) m * 5);

@@ -182,6 +182,16 @@ struct BlockPool {
 BlockPool g_pool;
 }  // namespace
 
+thread_local UploadTally t_uploads;
+void count_upload(const void *src, size_t bytes)
+{
+    cudaPointerAttributes pa;
+    if (cudaPointerGetAttributes(&pa, src) != cudaSuccess) { cudaGetLastError(); return; }
+    if (pa.type != cudaMemoryTypeHost && pa.type != cudaMemoryTypeUnregistered) return;
+    t_uploads.bytes += (long long) bytes;
+    t_uploads.largest = std::max(t_uploads.largest, (long long) bytes);
+}
+
 DeviceArena::~DeviceArena()
 {
     if (!blocks.empty()) cudaStreamSynchronize(st);
@@ -252,6 +262,15 @@ int build_visibility(const VisSource &src, int n, int m, cudaStream_t st, Device
         TRY(D.alloc(&V.obs_cam, (size_t) V.nvis)); TRY(D.alloc(&V.obs_pt, (size_t) V.nvis));
         vmask_fill_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(d_vmask, n, m, V.rowptr, V.obs_cam, V.obs_pt);
         BSFM_KERNEL_CHECK();
+    } else if (src.ours) {           // device CRS written by the library: used where it is, obs_pt from the row pointers
+        V.nvis = src.nvis;
+        V.rowptr = const_cast<int *>(src.vis_ptr);
+        if (V.nvis > 0) {
+            V.obs_cam = const_cast<int *>(src.vis_cam);
+            TRY(D.alloc(&V.obs_pt, (size_t) V.nvis));
+            csr_rows_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(V.rowptr, n, V.obs_pt);
+            BSFM_KERNEL_CHECK();
+        }
     } else {                         // sources 2 and 3: CRS arrays in host or device memory
         std::vector<int> h_rowptr, h_obs_cam;
         const int *rowptr = src.vis_ptr, *obs_cam = src.vis_cam;
@@ -267,9 +286,11 @@ int build_visibility(const VisSource &src, int n, int m, cudaStream_t st, Device
             V.nvis = src.nvis;
         }
         TRY(D.alloc(&V.rowptr, (size_t) n + 1));
+        note_upload(rowptr, ((size_t) n + 1) * sizeof(int));
         BSFM_CUDA_TRY(cudaMemcpyAsync(V.rowptr, rowptr, ((size_t) n + 1) * sizeof(int), cudaMemcpyDefault, st));
         if (V.nvis > 0) {
             TRY(D.alloc(&V.obs_cam, (size_t) V.nvis)); TRY(D.alloc(&V.obs_pt, (size_t) V.nvis));
+            note_upload(obs_cam, (size_t) V.nvis * sizeof(int));
             BSFM_CUDA_TRY(cudaMemcpyAsync(V.obs_cam, obs_cam, (size_t) V.nvis * sizeof(int), cudaMemcpyDefault, st));
         }
         if (host_mask) {

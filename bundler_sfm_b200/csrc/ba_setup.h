@@ -13,6 +13,14 @@
 namespace bsfm {
 namespace ba {
 
+// Host-to-device traffic of the calling thread while `on` (bsfm_run_sfm_outlier_loop reports it per round): every copy of
+// the BA setup whose source may be host memory goes through note_upload, which looks the pointer up and counts it when it
+// is.  Off, it costs one branch.
+struct UploadTally { bool on = false; long long bytes = 0, largest = 0; };
+extern thread_local UploadTally t_uploads;
+void count_upload(const void *src, size_t bytes);
+inline void note_upload(const void *src, size_t bytes) { if (t_uploads.on) count_upload(src, bytes); }
+
 // Device memory of one call, recycled through a process-wide pool of the current device's blocks.  The pool serves every
 // thread, so the destructor waits for `st`, the stream that uses the blocks, before returning them: an error return with
 // work in flight must not hand them to another call while that work still writes them.
@@ -32,6 +40,7 @@ struct DeviceArena {
     template <typename T> int upload(T **out, const void *src, size_t count)
     {
         TRY(alloc(out, count));
+        note_upload(src, count * sizeof(T));
         BSFM_CUDA_TRY(cudaMemcpyAsync((void *) *out, src, count * sizeof(T), cudaMemcpyDefault, st));
         return BSFM_OK;
     }
@@ -65,18 +74,27 @@ struct Visibility {
     int *cam_ptr = nullptr;   // m + 1: camera j's observations are cam_obs[cam_ptr[j] .. cam_ptr[j + 1])
 };
 // Where a call's visibility comes from: the dense n x m mask of the reference interface, or the caller's own CRS arrays
-// (the layout of Visibility::rowptr / obs_cam).  Host (pageable or pinned) or device pointers.
+// (the layout of Visibility::rowptr / obs_cam).  Host (pageable or pinned) or device pointers.  Inside the library also:
+// device CRS arrays the library wrote itself (`ours`: used in place, not checked again), and, for the solver, a Visibility
+// that has been built already (`built`).
 struct VisSource {
     const char *vmask = nullptr;
     const int32_t *vis_ptr = nullptr;   // n + 1
     const int32_t *vis_cam = nullptr;   // nvis
     int nvis = 0;
+    bool ours = false;
+    const struct Visibility *built = nullptr;
     static VisSource mask(const char *vmask) { VisSource s; s.vmask = vmask; return s; }
     static VisSource crs(const int32_t *vis_ptr, const int32_t *vis_cam, int nvis)
     {
         VisSource s; s.vis_ptr = vis_ptr; s.vis_cam = vis_cam; s.nvis = nvis; return s;
     }
-    bool present() const { return vmask || (vis_ptr && (vis_cam || nvis == 0)); }
+    static VisSource device_crs(const int32_t *vis_ptr, const int32_t *vis_cam, int nvis)
+    {
+        VisSource s = crs(vis_ptr, vis_cam, nvis); s.ours = true; return s;
+    }
+    static VisSource visibility(const Visibility *V) { VisSource s; s.built = V; return s; }
+    bool present() const { return built || vmask || (vis_ptr && (vis_cam || nvis == 0)); }
 };
 // Visibility from either source.  Synchronises `st` at most once: to learn nvis of a mask scanned on the device, or to
 // read the verdict on a caller's CRS.  A malformed CRS returns BSFM_ERR_ARG naming the lowest offending point

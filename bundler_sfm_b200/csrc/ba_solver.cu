@@ -8,7 +8,7 @@
 #include "common.h"
 #include "ba_kernels.cuh"
 #include "ba_chol_large.cuh"
-#include "ba_setup.h"
+#include "ba_loop.h"
 #include "../../include/bsfm_b200_ba.h"
 #include <cfloat>
 #include <chrono>
@@ -74,6 +74,9 @@ struct HostMarks {
 // stream, events and the pinned scalar blocks are created once per thread and device and reused: driver
 // calls that allocate (cudaMallocHost, cudaStreamCreate, ...) serialise on a global lock and cost more than
 // an LM iteration of the 50-camera configuration
+// Point constraints that are on the device already, in the layout of Problem::pt_constrained / pt_constraints / pt_weights
+struct DevicePointConstraints { const char *constrained; const double *constraints, *weights; };
+
 struct SolverCtx { int device = -1; cudaStream_t st = nullptr; cudaEvent_t ev_begin = nullptr, ev_end = nullptr; Scalars *h_sc = nullptr; double *h_mu = nullptr; };
 int solver_ctx(SolverCtx **out)
 {
@@ -135,7 +138,7 @@ struct Solve {
     int visibility(const VisSource &vis, const double *x);
     int upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, bool fisheye, const double *p, const double *fixed_pts,
                int use_constraints, const bsfm_camera_constraints_t *constraints,
-               int use_point_constraints, const bsfm_point_constraints_t *point_constraints);
+               int use_point_constraints, const bsfm_point_constraints_t *point_constraints, const DevicePointConstraints *dev_pc);
     int controller(int itmax, int verbose, const double opts[6], bool any_constraints, double *Vout);
     int export_blocks(double *Vout, double *Sout, double *Uout, double *Wout);
 
@@ -179,7 +182,8 @@ struct Solve {
 int Solve::visibility(const VisSource &vis, const double *x)
 {
     Visibility V;
-    TRY(build_visibility(vis, n, m, st, D, V));
+    if (vis.built) V = *vis.built;
+    else TRY(build_visibility(vis, n, m, st, D, V));
     nvis = V.nvis;
     P.nvis = nvis;
     nobs = nvis * 2;
@@ -195,7 +199,7 @@ int Solve::visibility(const VisSource &vis, const double *x)
 // model, calibrated cameras, fisheye cameras, constraints, work arrays and the initial parameters
 int Solve::upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, bool fisheye, const double *p, const double *fixed_pts,
                   int use_constraints, const bsfm_camera_constraints_t *constraints,
-                  int use_point_constraints, const bsfm_point_constraints_t *point_constraints)
+                  int use_point_constraints, const bsfm_point_constraints_t *point_constraints, const DevicePointConstraints *dev_pc)
 {
     TRY(D.upload(&P.R_init, model->R_init, (size_t) m * 9));
     if (model->f_fixed) TRY(D.upload(&P.f_fixed, model->f_fixed, (size_t) m));
@@ -241,7 +245,9 @@ int Solve::upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *ini
         TRY(D.upload(&P.cam_weights, h_cw.data(), h_cw.size()));
     }
     std::vector<char> h_pc; std::vector<double> h_pv, h_pw;
-    if (use_point_constraints) {
+    if (use_point_constraints && dev_pc) {
+        P.pt_constrained = dev_pc->constrained; P.pt_constraints = dev_pc->constraints; P.pt_weights = dev_pc->weights;
+    } else if (use_point_constraints) {
         if (!point_constraints) { set_error("use_point_constraints set but point_constraints == NULL"); return BSFM_ERR_ARG; }
         h_pc.resize(n); h_pv.resize((size_t) n * 3); h_pw.resize(n);
         for (int i = 0; i < n; i++) {
@@ -276,8 +282,10 @@ int Solve::upload(const bsfm_sfm_model_t *model, const bsfm_camera_params_t *ini
     BSFM_CUDA_TRY(cudaMemsetAsync(P.sc, 0, sizeof(Scalars), st));
     TRY(D.alloc(&d_mu, 1));
     P.mu = d_mu;
+    note_upload(p, (size_t) P.nlm * sizeof(double));
     BSFM_CUDA_TRY(cudaMemcpyAsync(d_p, p, (size_t) P.nlm * sizeof(double), cudaMemcpyDefault, st));
     if (mot) {
+        note_upload(fixed_pts, (size_t) n * 3 * sizeof(double));
         BSFM_CUDA_TRY(cudaMemcpyAsync(d_p + P.nlm, fixed_pts, (size_t) n * 3 * sizeof(double), cudaMemcpyDefault, st));
         BSFM_CUDA_TRY(cudaMemsetAsync(P.dp, 0, (size_t) P.nvars * sizeof(double), st));   // the points' increments stay 0
     }
@@ -442,13 +450,14 @@ int Solve::export_blocks(double *Vout, double *Sout, double *Uout, double *Wout)
 // Shared implementation of the two LM drivers (mot: see Solve).
 // init_params (nullable, m entries): the calibrated-camera fields (known_intrinsics, K_known, k_known) are read.
 // fisheye: project with sfm_project_point2_fisheye; init_params is required then, and its fisheye fields are read too.
+// dev_pc (nullable): the point constraints as device tables, taken in place of point_constraints.
 static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon, const VisSource &vis, double *p, int cnp, int pnp,
                        const double *x, const double *covx, int mnp,
                        const bsfm_sfm_model_t *model, const bsfm_camera_params_t *init_params, int fisheye, int jac_mode,
                        int itmax, int verbose, const double opts[6], double info[10],
                        int use_constraints, const bsfm_camera_constraints_t *constraints,
                        int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
-                       double *Vout, double *Sout, double *Uout, double *Wout)
+                       double *Vout, double *Sout, double *Uout, double *Wout, const DevicePointConstraints *dev_pc = nullptr)
 {
     clear_error();
     TRY(require_device());
@@ -485,7 +494,7 @@ static int levmar_impl(int mot, const double *fixed_pts, int n, int m, int mcon,
     TRY(build_schur_structure(S.P, st, S.D));
     if (!mot) TRY(apply_camera_order(S.P, cnp, st, S.D, S.band));      // large systems: S in the order that skips most of the factorisation
     S.HM.mark("Schur structure + camera order");
-    TRY(S.upload(model, init_params, fisheye != 0, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints));
+    TRY(S.upload(model, init_params, fisheye != 0, p, fixed_pts, use_constraints, constraints, use_point_constraints, point_constraints, dev_pc));
     S.PT.end();
     S.HM.mark("setup issued");
 
@@ -681,6 +690,149 @@ extern "C" int bsfm_ba_last_timing(float ms[6], int *iterations, int *launches)
     return BSFM_OK;
 }
 
+// run_sfm's handling of the cameras (lib/sfm-driver/sfm.c:652-696 packing, :721-754 constraints, :876-929 unpacking) and
+// its call of the solver (:705-714 options, :814-856), shared by run_sfm_impl and the outlier loop
+struct SfmCameras {
+    static constexpr double f_scale = 0.001, k_scale = 5.0;     // sfm.c:634-635 (TEST_FOCAL)
+    const int m, cnp, est_focal_length, undistort;
+    std::vector<double> R_init, f_fixed;
+    std::vector<bsfm_camera_constraints_t> constraints;
+    std::vector<char> cc; std::vector<double> cv, cw;
+    bsfm_sfm_model_t model;
+
+    SfmCameras(int num_cameras, int est_focal, int undist, int explicit_camera_centers)
+        : m(num_cameras), cnp((est_focal ? 7 : 6) + (undist ? 2 : 0)), est_focal_length(est_focal), undistort(undist),
+          R_init((size_t) num_cameras * 9), f_fixed(num_cameras)
+    {
+        model.est_focal_length = est_focal_length; model.undistort = undistort; model.explicit_camera_centers = explicit_camera_centers;
+        model.f_scale = f_scale; model.k_scale = k_scale; model.R_init = R_init.data(); model.f_fixed = f_fixed.data();
+    }
+    // cameras -> params (m * cnp), R_init, f_fixed and, with use_constraints, the scaled constraints
+    void pack(bsfm_camera_params_t *init_camera_params, double *params, int use_constraints)
+    {
+        for (int j = 0; j < m; j++) {                      // sfm.c:652-696
+            int c;
+            init_camera_params[j].f_scale = f_scale;
+            init_camera_params[j].k_scale = k_scale;
+            params[(size_t) cnp * j + 0] = init_camera_params[j].t[0];
+            params[(size_t) cnp * j + 1] = init_camera_params[j].t[1];
+            params[(size_t) cnp * j + 2] = init_camera_params[j].t[2];
+            params[(size_t) cnp * j + 3] = 0.0; params[(size_t) cnp * j + 4] = 0.0; params[(size_t) cnp * j + 5] = 0.0;
+            if (est_focal_length) { params[(size_t) cnp * j + 6] = init_camera_params[j].f * init_camera_params[j].f_scale; c = 7; }
+            else c = 6;
+            if (undistort) {
+                const double scale = init_camera_params[j].k_scale;
+                params[(size_t) cnp * j + c] = init_camera_params[j].k[0] * scale;
+                params[(size_t) cnp * j + c + 1] = init_camera_params[j].k[1] * scale;
+            }
+            memcpy(&R_init[(size_t) j * 9], init_camera_params[j].R, 9 * sizeof(double));
+            f_fixed[j] = init_camera_params[j].f;
+        }
+        if (!use_constraints) return;                      // sfm.c:721-754
+        constraints.resize(m);
+        cc.resize((size_t) m * cnp); cv.resize((size_t) m * cnp); cw.resize((size_t) m * cnp);
+        for (int i = 0; i < m; i++) {
+            char *c0 = &cc[(size_t) i * cnp]; double *v0 = &cv[(size_t) i * cnp]; double *w0 = &cw[(size_t) i * cnp];
+            memcpy(c0, init_camera_params[i].constrained, cnp);
+            memcpy(v0, init_camera_params[i].constraints, cnp * sizeof(double));
+            memcpy(w0, init_camera_params[i].weights, cnp * sizeof(double));
+            if (est_focal_length) { v0[6] *= f_scale; w0[6] *= (1.0 / (f_scale * f_scale)); }
+            if (undistort) {
+                // NOTE the reference indexes 7 and 8 unconditionally (sfm.c:745-751), i.e. it assumes est_focal_length;
+                // with est_focal_length == 0 that would be out of bounds for cnp == 8, so the k pair at 6,7 is used there.
+                const int k0 = est_focal_length ? 7 : 6;
+                v0[k0] *= k_scale; w0[k0] *= (1.0 / (k_scale * k_scale));
+                v0[k0 + 1] *= k_scale; w0[k0 + 1] *= (1.0 / (k_scale * k_scale));
+            }
+            constraints[i].constrained = c0; constraints[i].constraints = v0; constraints[i].weights = w0;
+        }
+    }
+    // a BSFM_ERR_* of the solver: nothing was solved; the caller's cameras get back the scale fields pack() set to 0.001 / 5
+    void restore_scales(bsfm_camera_params_t *init_camera_params) const
+    {
+        for (int j = 0; j < m; j++) { init_camera_params[j].f_scale = 1.0; init_camera_params[j].k_scale = 1.0; }
+    }
+    // host-side rot_update for the unpacking (sfm.c:876-929); same arithmetic as the device version
+    void unpack(const double *params, bsfm_camera_params_t *init_camera_params) const
+    {
+        for (int j = 0; j < m; j++) {
+            const double *dt = &params[(size_t) cnp * j + 0];
+            const double *w = &params[(size_t) cnp * j + 3];
+            int c;
+            init_camera_params[j].t[0] = dt[0]; init_camera_params[j].t[1] = dt[1]; init_camera_params[j].t[2] = dt[2];
+            {
+                double *R = init_camera_params[j].R, Rnew[9];
+                const double theta = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
+                if (theta != 0.0) {
+                    const double n0 = w[0] / theta, n1 = w[1] / theta, n2 = w[2] / theta;
+                    const double nx[9] = {0.0, -n2, n1, n2, 0.0, -n0, -n1, n0, 0.0};
+                    double nxsq[9], dR[9];
+                    for (int r = 0; r < 3; r++) for (int cc2 = 0; cc2 < 3; cc2++)
+                        nxsq[3 * r + cc2] = nx[3 * r] * nx[cc2] + nx[3 * r + 1] * nx[3 + cc2] + nx[3 * r + 2] * nx[6 + cc2];
+                    const double sinth = sin(theta), costh = cos(theta);
+                    for (int q = 0; q < 9; q++) dR[q] = (((q % 4 == 0) ? 1.0 : 0.0) + nx[q] * sinth) + nxsq[q] * (1.0 - costh);
+                    for (int r = 0; r < 3; r++) for (int cc2 = 0; cc2 < 3; cc2++)
+                        Rnew[3 * r + cc2] = dR[3 * r] * R[cc2] + dR[3 * r + 1] * R[3 + cc2] + dR[3 * r + 2] * R[6 + cc2];
+                    memcpy(R, Rnew, sizeof Rnew);
+                }
+            }
+            if (est_focal_length) { c = 7; init_camera_params[j].f = params[(size_t) cnp * j + 6] / init_camera_params[j].f_scale; }
+            else c = 6;
+            if (undistort) {
+                const double scale = init_camera_params[j].k_scale;
+                init_camera_params[j].k[0] = params[(size_t) cnp * j + c] / scale;
+                init_camera_params[j].k[1] = params[(size_t) cnp * j + c + 1] / scale;
+            }
+            init_camera_params[j].f_scale = 1.0;
+            init_camera_params[j].k_scale = 1.0;
+        }
+    }
+    // the solve of sfm.c:814-856 on packed parameters p = (cameras, points), host or device; prints run_sfm's two lines
+    // (:872-873) unless the solver returned a BSFM_ERR_*, which is passed on
+    int solve(int num_pts, int ncons, const VisSource &vis, double *p, const double *projections, const bsfm_camera_params_t *init_camera_params,
+              int use_constraints, int use_point_constraints, const bsfm_point_constraints_t *point_constraints,
+              const DevicePointConstraints *dev_pc, int fix_points, int optimize_for_fisheye, double eps2,
+              double *Vout, double *Sout, double *Uout, double *Wout, double info[10])
+    {
+        const double opts[6] = {1.0e-3, 1.0e-10, eps2, 1.0e-12, 0.0, 4.0e-2};   // sfm.c:705-714
+        const char *verb_env = getenv("BSFM_BA_VERBOSE");
+        const int verbosity = verb_env ? atoi(verb_env) : 3;          // VERBOSITY 3, MAX_ITERS 150 (sfm.c:814-815)
+        const size_t num_camera_params = (size_t) cnp * m;
+        int rc;
+        if (fix_points)     // sfm.c:843-849: motion-only BA, the points come from init_pts and stay as they are
+            rc = levmar_impl(1, p + num_camera_params, num_pts, m, ncons, vis, p, cnp, 3, projections,
+                             nullptr, 2, &model, init_camera_params, optimize_for_fisheye, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                             use_constraints, use_constraints ? constraints.data() : nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
+        else
+            rc = levmar_impl(0, nullptr, num_pts, m, ncons, vis, p, cnp, 3, projections, nullptr, 2,
+                             &model, init_camera_params, optimize_for_fisheye, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
+                             use_constraints, use_constraints ? constraints.data() : nullptr,
+                             use_point_constraints, point_constraints, Vout, Sout, Uout, Wout, dev_pc);
+        if (rc < -1) return rc;
+        printf("[run_sfm] Number of iterations: %d\n", (int) info[5]);   // sfm.c:872-873
+        printf("info[6] = %0.3f\n", info[6]);
+        return BSFM_OK;
+    }
+};
+
+// the point constraints of sfm.c:757-781 for points [0, num_pts)
+static void sfm_point_constraints(const bsfm_v3_t *pt_constraints, double pt_constraint_weight, int num_pts, std::vector<bsfm_point_constraints_t> &out)
+{
+    out.resize(num_pts);
+    for (int i = 0; i < num_pts; i++) {
+        const double *q = pt_constraints[i].p;
+        if (q[0] == 0.0 && q[1] == 0.0 && q[2] == 0.0) {
+            out[i].constrained = 0;
+            out[i].constraints[0] = out[i].constraints[1] = out[i].constraints[2] = 0.0;
+            out[i].weight = 0.0;
+        } else {
+            out[i].constrained = 1;
+            out[i].weight = pt_constraint_weight;
+            out[i].constraints[0] = q[0]; out[i].constraints[1] = q[1]; out[i].constraints[2] = q[2];
+        }
+    }
+}
+
 // == run_sfm, lib/sfm-driver/sfm.c:592-1003, on either visibility source (bsfm_run_sfm, bsfm_run_sfm_crs)
 static int run_sfm_impl(int num_pts, int num_cameras, int ncons, const VisSource &vis, double *projections,
                         int est_focal_length, int const_focal_length, int undistort, int explicit_camera_centers,
@@ -697,133 +849,26 @@ static int run_sfm_impl(int num_pts, int num_cameras, int ncons, const VisSource
         set_error("bsfm_run_sfm: bad arguments"); return BSFM_ERR_ARG;
     }
 
-    const double f_scale = 0.001, k_scale = 5.0;                 // sfm.c:634-635 (TEST_FOCAL)
-    int cnp = est_focal_length ? 7 : 6;
-    if (undistort) cnp += 2;
+    SfmCameras C(num_cameras, est_focal_length, undistort, explicit_camera_centers);
+    const int cnp = C.cnp;
     const int num_camera_params = cnp * num_cameras;
     const size_t num_params = (size_t) num_camera_params + 3 * (size_t) num_pts;
     std::vector<double> params(num_params);
-    std::vector<double> R_init((size_t) num_cameras * 9), f_fixed(num_cameras);
-    for (int j = 0; j < num_cameras; j++) {                      // sfm.c:652-696
-        int c;
-        init_camera_params[j].f_scale = f_scale;
-        init_camera_params[j].k_scale = k_scale;
-        params[(size_t) cnp * j + 0] = init_camera_params[j].t[0];
-        params[(size_t) cnp * j + 1] = init_camera_params[j].t[1];
-        params[(size_t) cnp * j + 2] = init_camera_params[j].t[2];
-        params[(size_t) cnp * j + 3] = 0.0; params[(size_t) cnp * j + 4] = 0.0; params[(size_t) cnp * j + 5] = 0.0;
-        if (est_focal_length) { params[(size_t) cnp * j + 6] = init_camera_params[j].f * init_camera_params[j].f_scale; c = 7; }
-        else c = 6;
-        if (undistort) {
-            const double scale = init_camera_params[j].k_scale;
-            params[(size_t) cnp * j + c] = init_camera_params[j].k[0] * scale;
-            params[(size_t) cnp * j + c + 1] = init_camera_params[j].k[1] * scale;
-        }
-        memcpy(&R_init[(size_t) j * 9], init_camera_params[j].R, 9 * sizeof(double));
-        f_fixed[j] = init_camera_params[j].f;
-    }
+    C.pack(init_camera_params, params.data(), use_constraints);
     for (int i = 0; i < num_pts; i++)                            // sfm.c:698-703
         for (int q = 0; q < 3; q++) params[(size_t) num_camera_params + 3 * (size_t) i + q] = init_pts[i].p[q];
-
-    double opts[6] = {1.0e-3, 1.0e-10, eps2, 1.0e-12, 0.0, 4.0e-2};   // sfm.c:705-714
     double info[10] = {0};
-
-    std::vector<bsfm_camera_constraints_t> constraints;
-    std::vector<char> cc; std::vector<double> cv, cw;
-    if (use_constraints) {                                       // sfm.c:721-754
-        constraints.resize(num_cameras);
-        cc.resize((size_t) num_cameras * cnp); cv.resize((size_t) num_cameras * cnp); cw.resize((size_t) num_cameras * cnp);
-        for (int i = 0; i < num_cameras; i++) {
-            char *c0 = &cc[(size_t) i * cnp]; double *v0 = &cv[(size_t) i * cnp]; double *w0 = &cw[(size_t) i * cnp];
-            memcpy(c0, init_camera_params[i].constrained, cnp);
-            memcpy(v0, init_camera_params[i].constraints, cnp * sizeof(double));
-            memcpy(w0, init_camera_params[i].weights, cnp * sizeof(double));
-            if (est_focal_length) { v0[6] *= f_scale; w0[6] *= (1.0 / (f_scale * f_scale)); }
-            if (undistort) {
-                // NOTE the reference indexes 7 and 8 unconditionally (sfm.c:745-751), i.e. it assumes est_focal_length;
-                // with est_focal_length == 0 that would be out of bounds for cnp == 8, so the k pair at 6,7 is used there.
-                const int k0 = est_focal_length ? 7 : 6;
-                v0[k0] *= k_scale; w0[k0] *= (1.0 / (k_scale * k_scale));
-                v0[k0 + 1] *= k_scale; w0[k0 + 1] *= (1.0 / (k_scale * k_scale));
-            }
-            constraints[i].constrained = c0; constraints[i].constraints = v0; constraints[i].weights = w0;
-        }
-    }
     std::vector<bsfm_point_constraints_t> point_constraints;
     if (use_point_constraints) {                                 // sfm.c:757-781
         if (!pt_constraints) { set_error("bsfm_run_sfm: use_point_constraints without points_constraints"); return BSFM_ERR_ARG; }
-        point_constraints.resize(num_pts);
-        for (int i = 0; i < num_pts; i++) {
-            const double *q = pt_constraints[i].p;
-            if (q[0] == 0.0 && q[1] == 0.0 && q[2] == 0.0) {
-                point_constraints[i].constrained = 0;
-                point_constraints[i].constraints[0] = point_constraints[i].constraints[1] = point_constraints[i].constraints[2] = 0.0;
-                point_constraints[i].weight = 0.0;
-            } else {
-                point_constraints[i].constrained = 1;
-                point_constraints[i].weight = pt_constraint_weight;
-                point_constraints[i].constraints[0] = q[0]; point_constraints[i].constraints[1] = q[1]; point_constraints[i].constraints[2] = q[2];
-            }
-        }
+        sfm_point_constraints(pt_constraints, pt_constraint_weight, num_pts, point_constraints);
     }
-
-    bsfm_sfm_model_t model;
-    model.est_focal_length = est_focal_length; model.undistort = undistort; model.explicit_camera_centers = explicit_camera_centers;
-    model.f_scale = f_scale; model.k_scale = k_scale; model.R_init = R_init.data(); model.f_fixed = f_fixed.data();
-
-    const char *verb_env = getenv("BSFM_BA_VERBOSE");
-    const int verbosity = verb_env ? atoi(verb_env) : 3;          // VERBOSITY 3, MAX_ITERS 150 (sfm.c:814-815)
-    int rc;
-    if (fix_points)     // sfm.c:843-849: motion-only BA, the points come from init_pts and stay as they are
-        rc = levmar_impl(1, params.data() + num_camera_params, num_pts, num_cameras, ncons, vis, params.data(), cnp, 3, projections,
-                         nullptr, 2, &model, init_camera_params, optimize_for_fisheye, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
-                         use_constraints, use_constraints ? constraints.data() : nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
-    else
-        rc = levmar_impl(0, nullptr, num_pts, num_cameras, ncons, vis, params.data(), cnp, 3, projections, nullptr, 2,
-                         &model, init_camera_params, optimize_for_fisheye, BSFM_BA_JAC_FD, 150, verbosity, opts, info,
-                         use_constraints, use_constraints ? constraints.data() : nullptr,
-                         use_point_constraints, use_point_constraints ? point_constraints.data() : nullptr,
-                         Vout, Sout, Uout, Wout);
-    if (rc < -1) {              // BSFM_ERR_*: nothing was solved; the caller's cameras get their scale fields back (they were set
-        for (int j = 0; j < num_cameras; j++) { init_camera_params[j].f_scale = 1.0; init_camera_params[j].k_scale = 1.0; }   // to 0.001 / 5 above)
-        return rc;
-    }
-    printf("[run_sfm] Number of iterations: %d\n", (int) info[5]);   // sfm.c:872-873
-    printf("info[6] = %0.3f\n", info[6]);
+    const int rc = C.solve(num_pts, ncons, vis, params.data(), projections, init_camera_params, use_constraints, use_point_constraints,
+                           use_point_constraints ? point_constraints.data() : nullptr, nullptr, fix_points, optimize_for_fisheye, eps2,
+                           Vout, Sout, Uout, Wout, info);
+    if (rc != BSFM_OK) { C.restore_scales(init_camera_params); return rc; }
     if (info_out) memcpy(info_out, info, sizeof info);
-
-    // host-side rot_update for the unpacking (sfm.c:876-929); same arithmetic as the device version
-    for (int j = 0; j < num_cameras; j++) {
-        const double *dt = &params[(size_t) cnp * j + 0];
-        const double *w = &params[(size_t) cnp * j + 3];
-        int c;
-        init_camera_params[j].t[0] = dt[0]; init_camera_params[j].t[1] = dt[1]; init_camera_params[j].t[2] = dt[2];
-        {
-            double *R = init_camera_params[j].R, Rnew[9];
-            const double theta = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-            if (theta != 0.0) {
-                const double n0 = w[0] / theta, n1 = w[1] / theta, n2 = w[2] / theta;
-                const double nx[9] = {0.0, -n2, n1, n2, 0.0, -n0, -n1, n0, 0.0};
-                double nxsq[9], dR[9];
-                for (int r = 0; r < 3; r++) for (int cc2 = 0; cc2 < 3; cc2++)
-                    nxsq[3 * r + cc2] = nx[3 * r] * nx[cc2] + nx[3 * r + 1] * nx[3 + cc2] + nx[3 * r + 2] * nx[6 + cc2];
-                const double sinth = sin(theta), costh = cos(theta);
-                for (int q = 0; q < 9; q++) dR[q] = (((q % 4 == 0) ? 1.0 : 0.0) + nx[q] * sinth) + nxsq[q] * (1.0 - costh);
-                for (int r = 0; r < 3; r++) for (int cc2 = 0; cc2 < 3; cc2++)
-                    Rnew[3 * r + cc2] = dR[3 * r] * R[cc2] + dR[3 * r + 1] * R[3 + cc2] + dR[3 * r + 2] * R[6 + cc2];
-                memcpy(R, Rnew, sizeof Rnew);
-            }
-        }
-        if (est_focal_length) { c = 7; init_camera_params[j].f = params[(size_t) cnp * j + 6] / init_camera_params[j].f_scale; }
-        else c = 6;
-        if (undistort) {
-            const double scale = init_camera_params[j].k_scale;
-            init_camera_params[j].k[0] = params[(size_t) cnp * j + c] / scale;
-            init_camera_params[j].k[1] = params[(size_t) cnp * j + c + 1] / scale;
-        }
-        init_camera_params[j].f_scale = 1.0;
-        init_camera_params[j].k_scale = 1.0;
-    }
+    C.unpack(params.data(), init_camera_params);
     for (int i = 0; i < num_pts; i++)
         for (int q = 0; q < 3; q++) init_pts[i].p[q] = params[(size_t) num_camera_params + 3 * (size_t) i + q];
     return BSFM_OK;
@@ -877,4 +922,143 @@ extern "C" int bsfm_run_sfm_crs_fe(int num_pts, int num_cameras, int ncons, cons
                         const_focal_length, undistort, explicit_camera_centers, init_camera_params, init_pts, use_constraints,
                         use_point_constraints, pt_constraints, pt_constraint_weight, fix_points, optimize_for_fisheye, eps2,
                         Vout, Sout, Uout, Wout, info_out, true);
+}
+
+// == the do / while of BundlerApp::RunSFM_SBA (src/Bundle.cpp:588-913): solve, outlier pass, removal, until a round removes
+// at most min_outliers points.  The scene goes to the device once and is compacted there between rounds (ba_loop.cu); a
+// round's solve and outlier pass share one Visibility.  Per round the host sends the packed cameras and their tables and
+// reads back the cameras, the m x 5 statistics and three counts.
+extern "C" int bsfm_run_sfm_outlier_loop(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                                         const double *projections, int est_focal_length, int const_focal_length, int undistort,
+                                         int explicit_camera_centers, bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                                         int use_constraints, int use_point_constraints, bsfm_v3_t *pt_constraints,
+                                         double pt_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                                         int remove_outliers, int min_outliers, int min_points,
+                                         double min_proj_error_threshold, double max_proj_error_threshold,
+                                         int32_t *pt_round, double *pt_error, double *cam_stats,
+                                         bsfm_sfm_round_t *rounds, int rounds_cap, double *mean_error)
+{
+    clear_error();
+    TRY(require_device());
+    if (est_focal_length && const_focal_length) { set_error("bsfm_run_sfm_outlier_loop: const_focal_length is not implemented (nor in the reference, sfm.c:518-521)"); return BSFM_ERR_UNSUPPORTED; }
+    const VisSource caller = VisSource::crs(vis_ptr, vis_cam, nvis);
+    if (num_pts <= 0 || num_cameras <= 0 || !caller.present() || (nvis > 0 && !projections) || !init_camera_params || !init_pts || !pt_round || !pt_error ||
+        rounds_cap < 0 || (rounds_cap > 0 && !rounds) || !mean_error) {
+        set_error("bsfm_run_sfm_outlier_loop: bad arguments"); return BSFM_ERR_ARG;
+    }
+    if (use_point_constraints && !pt_constraints) { set_error("bsfm_run_sfm_outlier_loop: use_point_constraints without points_constraints"); return BSFM_ERR_ARG; }
+
+    const int m = num_cameras;
+    SfmCameras C(m, est_focal_length, undistort, explicit_camera_centers);
+    const int ncp = C.cnp * m;
+    SolverCtx *ctx;
+    TRY(solver_ctx(&ctx));
+    const cudaStream_t st = ctx->st;
+    struct TallyGuard { TallyGuard() { t_uploads = UploadTally(); t_uploads.on = true; } ~TallyGuard() { t_uploads.on = false; } } tally;
+    DeviceArena D(st);      // the scene: lives until the loop ends
+
+    // the caller's scene, checked like bsfm_run_sfm_crs checks it
+    Visibility V0;
+    TRY(build_visibility(caller, num_pts, m, st, D, V0));
+    if (V0.nvis <= 0) { set_error("bsfm_run_sfm_outlier_loop: no point has a view"); return BSFM_ERR_ARG; }
+    LoopFull full;
+    double *d_proj0;
+    TRY(D.upload(&d_proj0, projections, (size_t) nvis * 2));
+    TRY(D.upload(&full.pts, init_pts, (size_t) num_pts * 3));
+    TRY(D.alloc(&full.pt_round, (size_t) num_pts)); TRY(D.alloc(&full.pt_error, (size_t) num_pts));
+    // protected points, by ORIGINAL index (Bundle.cpp:800-806), and the solver's point constraints, which it reads by the
+    // index of the ROUND (the reference passes m_point_constraints to run_sfm as it is, Bundle.cpp:651, sfm.c:757-781):
+    // neither array is ever compacted, a round's solve takes the first n entries of the tables
+    DevicePointConstraints dpc = {nullptr, nullptr, nullptr};
+    if (use_point_constraints) {
+        std::vector<char> h_prot(num_pts), h_pc(num_pts);
+        std::vector<double> h_pv((size_t) num_pts * 3), h_pw(num_pts);
+        std::vector<bsfm_point_constraints_t> pc;
+        sfm_point_constraints(pt_constraints, pt_constraint_weight, num_pts, pc);
+        for (int i = 0; i < num_pts; i++) {
+            h_prot[i] = pt_constraints[i].p[0] != 0.0;
+            h_pc[i] = pc[i].constrained ? 1 : 0;
+            for (int q = 0; q < 3; q++) h_pv[(size_t) i * 3 + q] = pc[i].constraints[q];
+            h_pw[i] = pc[i].weight;
+        }
+        char *d_prot, *d_pc; double *d_pv, *d_pw;
+        TRY(D.upload(&d_prot, h_prot.data(), h_prot.size())); TRY(D.upload(&d_pc, h_pc.data(), h_pc.size()));
+        TRY(D.upload(&d_pv, h_pv.data(), h_pv.size())); TRY(D.upload(&d_pw, h_pw.data(), h_pw.size()));
+        full.prot = d_prot;
+        dpc.constrained = d_pc; dpc.constraints = d_pv; dpc.weights = d_pw;
+        BSFM_CUDA_TRY(cudaStreamSynchronize(st));     // the host vectors go out of scope
+    }
+    LoopScene half[2];
+    TRY(alloc_loop_scene(half[0], num_pts, nvis, ncp, use_point_constraints != 0, D));
+    TRY(alloc_loop_scene(half[1], num_pts, nvis, ncp, use_point_constraints != 0, D));
+    int counts[3];
+    TRY(loop_compact_entry(num_pts, ncp, V0.rowptr, V0.obs_cam, d_proj0, full, half[0], counts, st, D));
+
+    std::vector<double> cam_params(ncp), stats((size_t) m * 5);
+    int cur = 0, nrounds = 0, total_outliers = 0, num_outliers = 0, rc = BSFM_OK;
+    long long counted = 0;
+    *mean_error = 0.0;
+    do {
+        if (num_pts - total_outliers < min_points) {          // Bundle.cpp:588-595
+            printf("[RunSFM] Too few points remaining, exiting!\n");
+            fflush(stdout);
+            *mean_error = DBL_MAX;
+            break;
+        }
+        LoopScene &S = half[cur];
+        bsfm_sfm_round_t R;
+        memset(&R, 0, sizeof R);
+        R.num_pts = S.n; R.nvis = S.nvis;
+        DeviceArena RD(st);     // the round: its Visibility, the outlier pass and the scans
+        rc = [&]() -> int {
+            Visibility V;
+            TRY(build_visibility(VisSource::device_crs(S.vis_ptr, S.vis_cam, S.nvis), S.n, m, st, RD, V));
+            C.pack(init_camera_params, cam_params.data(), use_constraints);
+            note_upload(cam_params.data(), (size_t) ncp * sizeof(double));
+            BSFM_CUDA_TRY(cudaMemcpyAsync(S.p, cam_params.data(), (size_t) ncp * sizeof(double), cudaMemcpyHostToDevice, st));
+            const int src = C.solve(S.n, ncons, VisSource::visibility(&V), S.p, S.proj, init_camera_params, use_constraints, use_point_constraints,
+                                    nullptr, use_point_constraints ? &dpc : nullptr, fix_points, optimize_for_fisheye, eps2,
+                                    nullptr, nullptr, nullptr, nullptr, R.info);
+            if (src != BSFM_OK) { C.restore_scales(init_camera_params); return src; }
+            BSFM_CUDA_TRY(cudaMemcpyAsync(cam_params.data(), S.p, (size_t) ncp * sizeof(double), cudaMemcpyDeviceToHost, st));
+            BSFM_CUDA_TRY(cudaStreamSynchronize(st));
+            C.unpack(cam_params.data(), init_camera_params);
+
+            OutlierCams T;
+            OutlierPass pass;
+            TRY(upload_outlier_cams(init_camera_params, m, optimize_for_fisheye, RD, T));
+            TRY(outliers_core(V, S.n, m, T, S.p + ncp, S.proj, undistort, min_proj_error_threshold, max_proj_error_threshold, S.prot, st, RD, pass));
+            BSFM_CUDA_TRY(cudaMemcpyAsync(stats.data(), pass.stats, stats.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+            TRY(loop_compact_round(m, ncp, nrounds, remove_outliers ? 1 : 0, S, pass, full, half[cur ^ 1], counts, st, RD));
+            return BSFM_OK;
+        }();
+        if (rc != BSFM_OK) break;
+        double tot = 0.0, cnt = 0.0;      // Bundle.cpp:790-791, :852-856: sum of the per-camera sums / number of observations
+        for (int j = 0; j < m; j++) if (stats[5 * (size_t) j] > 0) { tot += stats[5 * (size_t) j + 1] * stats[5 * (size_t) j]; cnt += stats[5 * (size_t) j]; }
+        R.global_mean = tot / cnt;
+        *mean_error = R.global_mean;
+        if (cam_stats) memcpy(cam_stats, stats.data(), stats.size() * sizeof(double));
+        num_outliers = counts[2];
+        R.num_outliers = num_outliers;
+        R.removed = remove_outliers ? 1 : 0;
+        R.h2d_bytes = t_uploads.bytes - counted; R.h2d_largest = t_uploads.largest;
+        counted = t_uploads.bytes; t_uploads.largest = 0;
+        if (nrounds < rounds_cap) rounds[nrounds] = R;
+        nrounds++;
+        if (!remove_outliers) break;                          // Bundle.cpp:911
+        total_outliers += num_outliers;
+        cur ^= 1;
+    } while (num_outliers > min_outliers);                    // Bundle.cpp:913
+
+    // what the completed rounds left, also on an error return
+    const char *failed = rc != BSFM_OK ? last_error() : nullptr;
+    char keep_msg[1024];
+    if (failed) snprintf(keep_msg, sizeof keep_msg, "%s", failed);
+    cudaMemcpyAsync(init_pts, full.pts, (size_t) num_pts * 3 * sizeof(double), cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(pt_round, full.pt_round, (size_t) num_pts * sizeof(int), cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(pt_error, full.pt_error, (size_t) num_pts * sizeof(double), cudaMemcpyDeviceToHost, st);
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (rc != BSFM_OK) { set_error("%s", keep_msg); return rc; }
+    if (e != cudaSuccess) { set_error("bsfm_run_sfm_outlier_loop: copying the results back: %s", cudaGetErrorString(e)); return BSFM_ERR_CUDA; }
+    return nrounds;
 }

@@ -249,6 +249,38 @@ def crs_scene(scene):
     return out
 
 
+def inject_outliers(scene, count, seed, displacement=50.0, all_views=False, candidates=None, camera=None):
+    """a copy of a (dense or CRS) scene in which `count` seeded points are gross outliers: the measurement of one of
+    their views (seeded), or of all of them, is moved by `displacement` to 2 * `displacement` pixels in a seeded
+    direction.  The default 50 px is far above the largest threshold the outlier pass can use (16 px with Bundler's
+    settings).  candidates: the points to choose from (default: every point with a view).  camera: choose among the
+    points this camera sees and move their view in it (a camera with more than a fifth of its views displaced raises its
+    own threshold, which is how a scene is made to take several rounds).  Returns (scene, chosen points, ascending)."""
+    rng = np.random.default_rng(seed)
+    if "vis_ptr" in scene:
+        ptr = np.asarray(scene["vis_ptr"], dtype=np.int64)
+    else:
+        ptr = np.concatenate([[0], np.cumsum(np.count_nonzero(scene["vmask"], axis=1))])
+    views = np.diff(ptr)
+    pool = np.nonzero(views > 0)[0] if candidates is None else np.asarray(candidates)
+    if camera is not None:
+        from .bundle import observations
+        obs_pt, obs_cam = observations(scene)
+        in_cam = np.nonzero(obs_cam == camera)[0]
+        cam_view = dict(zip(obs_pt[in_cam].tolist(), in_cam.tolist()))
+        pool = np.array([i for i in pool if i in cam_view], dtype=np.int64)
+    chosen = np.sort(rng.choice(pool, size=count, replace=False))
+    proj = np.array(scene["projections"], dtype=np.float64)
+    for i in chosen:
+        obs = np.arange(ptr[i], ptr[i + 1]) if all_views else [cam_view[int(i)] if camera is not None else ptr[i] + rng.integers(views[i])]
+        for o in obs:
+            ang = rng.uniform(0.0, 2.0 * np.pi)
+            proj[o] += rng.uniform(displacement, 2.0 * displacement) * np.array([np.cos(ang), np.sin(ang)])
+    out = dict(scene)
+    out["projections"] = proj
+    return out, chosen
+
+
 def ki_kwargs(scene):
     """the calibration keywords (known, K_known, k_known) of a scene for run_sfm / call_run_sfm / reprojection_rmse /
     reprojection_outliers; empty for a scene without calibrated cameras"""

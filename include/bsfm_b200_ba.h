@@ -255,6 +255,68 @@ int bsfm_reprojection_outliers_crs_fe(int num_pts, int num_cameras, const int32_
                                       const char *pt_protected, double *cam_stats, double *obs_dist,
                                       int32_t *outliers, double *outlier_errors, int cap, double *global_mean);
 
+/* One round of bsfm_run_sfm_outlier_loop */
+typedef struct {
+    int32_t num_pts;        /* points solved this round (the reference's nz_count, src/Bundle.cpp:613-637) */
+    int32_t nvis;           /* observations solved this round */
+    int32_t num_outliers;   /* points flagged by this round's outlier pass */
+    int32_t removed;        /* 1 when they were removed (remove_outliers != 0) */
+    double  info[10];       /* sba's info[] of this round's solve */
+    double  global_mean;    /* "[RunSFM] Global mean reprojection error" of this round (:852-856) */
+    int64_t h2d_bytes;      /* bytes the round's setup (scene, cameras, tables, structure) copied from host to device ... */
+    int64_t h2d_largest;    /* ... and its largest single copy.  Round 0 includes the upload of the scene; the 8-byte */
+                            /* damping term the controller sends per LM try is not counted. */
+} bsfm_sfm_round_t;
+
+/* The solve / outlier-removal loop of BundlerApp::RunSFM_SBA (src/Bundle.cpp:568-919) as one call: bsfm_run_sfm_crs_fe,
+ * bsfm_reprojection_outliers_crs_fe and the removal of the flagged points, repeated until a round flags at most
+ * min_outliers points.  The scene is uploaded once and stays on the device between rounds; a round is bit-identical to
+ * the two separate calls on the same inputs.  After the first round the host sends only the cameras (packed parameters and
+ * the tables the kernels read) and reads back the cameras, the per-camera statistics and three counts.
+ *   visibility   CRS only (see bsfm_run_sfm_crs; host or device pointers), checked once with the same BSFM_ERR_ARG
+ *                messages.  RunSFM_SBA holds tracks (pt_views); the dense mask it builds from them every round
+ *                (:606-623) is the cost this entry avoids.
+ *   dropping     before every round, points without views leave the problem and the others are renumbered densely in
+ *                ascending original index (remap, :614-636) -- on entry too (pt_round = -2).  init_pts[i] of a point that
+ *                was dropped keeps the value it had when it was last solved (:905-909).
+ *   loop control at the top of every round, num_pts - (outliers removed so far) < min_points, on the ORIGINAL num_pts,
+ *                prints "[RunSFM] Too few points remaining, exiting!" and ends the loop with *mean_error = DBL_MAX
+ *                (:588-595).  Otherwise the loop runs while the last round removed more than min_outliers points (:913);
+ *                a round that flags fewer still removes them, then stops.  remove_outliers == 0 runs exactly one round and
+ *                removes nothing (:858, :911).  Bundler's values: min_outliers 40, min_points 20.
+ *   protection   a point with use_point_constraints && points_constraints[i].p[0] != 0.0, i its ORIGINAL index, is never
+ *                flagged (:800-806).
+ *   QUIRK        the reference hands m_point_constraints to run_sfm as it is (:651), so the SOLVE reads
+ *                points_constraints[q] for the index q a point has in that round (sfm.c:757-781), while the protection
+ *                test reads the original index.  Once a point below a constrained one has been removed (or had no view on
+ *                entry) the two disagree: the constraint then pulls on the point that took the constrained point's place.
+ *                This entry does what the reference does; points_constraints is never compacted.
+ *   outliers     whole points: all views of a flagged point go away (:871-889).  Flagging, thresholds, the reported error
+ *                (first flagging camera) and the fisheye DistortPoint step are those of bsfm_reprojection_outliers_crs_fe
+ *                with estimate_distortion = undistort (:647, :739).
+ *   solver       fix_points = 1 runs the motion-only solver every round; optimize_for_fisheye is honoured;
+ *                const_focal_length is refused as in bsfm_run_sfm.  V/S/U/W are not exported: Bundler asks for them only
+ *                on the two-camera first solve (src/Bundle.cpp:2150-2154), which goes to bsfm_run_sfm.  k_inv
+ *                (InvertDistortion, :680-705) needs image sizes and stays with the caller.  A solve that ends with
+ *                SBA_ERROR continues to the outlier pass, like run_sfm.
+ *   prints       per round the two lines of bsfm_run_sfm, and the too-few-points line.
+ * Outputs: init_camera_params, init_pts (in/out, by original index); pt_round[num_pts] = the round (0-based) whose pass
+ * removed the point, -1 kept, -2 no view on entry; pt_error[num_pts] = the reported reprojection error of a removed point
+ * (0 otherwise); cam_stats (nullable, num_cameras x 5, layout of bsfm_reprojection_outliers) of the LAST round;
+ * rounds[min(rounds_cap, return value)]; *mean_error = RunSFM_SBA's return value, the mean distance over the observations
+ * of the last round (its global_mean; the reference adds the same distances in one running sum), 0 when no round ran.
+ * Returns the number of rounds run (>= 0, may exceed rounds_cap) or a negative BSFM_ERR_*; then the outputs hold what
+ * the completed rounds left.                                                                                          */
+int bsfm_run_sfm_outlier_loop(int num_pts, int num_cameras, int ncons, const int32_t *vis_ptr, const int32_t *vis_cam, int nvis,
+                              const double *projections, int est_focal_length, int const_focal_length, int undistort,
+                              int explicit_camera_centers, bsfm_camera_params_t *init_camera_params, bsfm_v3_t *init_pts,
+                              int use_constraints, int use_point_constraints, bsfm_v3_t *points_constraints,
+                              double point_constraint_weight, int fix_points, int optimize_for_fisheye, double eps2,
+                              int remove_outliers, int min_outliers, int min_points,
+                              double min_proj_error_threshold, double max_proj_error_threshold,
+                              int32_t *pt_round, double *pt_error, double *cam_stats,
+                              bsfm_sfm_round_t *rounds, int rounds_cap, double *mean_error);
+
 /* == sba_Axb_Chol (lib/sba-1.5/sba_lapack.c:374-485, called at sba_levmar.c:1343): x = A^-1 B for a symmetric
  * positive definite m x m matrix (dpotrf + dpotrs in the reference).  A, B, x: host or device pointers; A and B are
  * NOT modified (the reference overwrites them when iscolmaj == 1).  Returns 1 on success, 0 when A is not positive
